@@ -1,2 +1,2 @@
-"""abyss_b200: B200-native Bloom-filter de Bruijn graph unitig stage (abyss-bloom-dbg path)."""
+"""abyss_b200: H100-native (sm_90a) Bloom-filter de Bruijn graph unitig stage (abyss-bloom-dbg path)."""
 __version__ = "0.1.0"

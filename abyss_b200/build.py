@@ -1,9 +1,9 @@
-"""In-tree build of libabyssb200.so (hand-written sm_100a CUDA behind the C ABI in include/abyss_b200.h).
+"""In-tree build of libabyssb200.so (hand-written sm_90a CUDA for the H100 behind the C ABI in include/abyss_b200.h).
 
     python -m abyss_b200.build [--force]
 
-nvcc cross-compiles for sm_100a without a GPU; the .so is git-ignored but travels with the
-repo snapshot to the GPU box.
+nvcc cross-compiles for sm_90a without a GPU; the .so and the host programs are git-ignored build products under
+abyss_b200/lib/.
 """
 from __future__ import annotations
 
@@ -22,8 +22,9 @@ SOURCES = {
     "abb_assemble.cu": ["abb_common.h", "abb_device.cuh", "abb_walk.cuh", "../../include/abyss_b200.h"],
     "abb_overlap.cu": ["abb_common.h", "abb_device.cuh", "abb_overlap.cuh", "../../include/abyss_b200.h"],
 }
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    *ARCH, "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC,-Wall,-Wno-unused-function", "--expt-relaxed-constexpr", "-ccbin", "g++",
 ]
 OBJDIR = os.path.join(LIBDIR, "obj")
@@ -33,7 +34,7 @@ CLIS = (("abyss-bloom-dbg", "abyss_bloom_dbg.cc"), ("abyss-bloom", "abyss_bloom.
 
 def _digest(paths) -> str:
     import hashlib
-    h = hashlib.sha1()
+    h = hashlib.sha1(" ".join(FLAGS).encode())  # a change of target architecture or flags rebuilds everything
     for p in sorted(paths):
         if os.path.exists(p):
             h.update(os.path.basename(p).encode())
@@ -97,7 +98,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
             print(out)
     objs = [o for o, _ in _objects().values()]
     if force or _stale(LIB, objs):
-        cmd = [NVCC, "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-cudart", "static", "-Xcompiler", "-fPIC", "-o", LIB, *objs,
+        cmd = [NVCC, *ARCH, "-shared", "-cudart", "static", "-Xcompiler", "-fPIC", "-o", LIB, *objs,
                "-ldl"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:

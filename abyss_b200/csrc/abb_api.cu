@@ -51,7 +51,7 @@ int select_device(int device)
 	}
 	ABB_CUDA(cudaSetDevice(device));
 	// tuning knob: ABB_L2_FETCH=32 asks L2 to fetch 32 B sectors from HBM (cudaLimitMaxL2FetchGranularity).
-	// Measured on B200: no gain for the random 1-byte Bloom accesses (0.85 vs 0.90 G k-mers/s), so off by default.
+	// Off by default: the Bloom accesses are random single bytes, and the hardware's default fetch size is kept.
 	static int fetch = -1;
 	if (fetch < 0) {
 		const char* e = getenv("ABB_L2_FETCH");
@@ -376,7 +376,7 @@ int launch_hash(abb_filter* f, unsigned k, const uint8_t* d_care, const uint8_t*
 	const uint64_t n = r1 - r0;
 	if (n == 0)
 		return ABB_OK;
-	int sms = 148, dev = 0;
+	int sms = 132, dev = 0;
 	cudaGetDevice(&dev);
 	cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
 	const unsigned grid = (unsigned)std::min<uint64_t>((n + kHashWarps - 1) / kHashWarps, (uint64_t)sms * 32);
@@ -414,7 +414,7 @@ int launch_hash_segments(unsigned k, const uint8_t* d_care, const uint8_t* d_bas
 {
 	if (n_segs == 0)
 		return ABB_OK;
-	int sms = 148, dev = 0;
+	int sms = 132, dev = 0;
 	cudaGetDevice(&dev);
 	cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
 	const unsigned grid = (unsigned)std::min<uint64_t>((n_segs + kHashWarps - 1) / kHashWarps, (uint64_t)sms * 32);
@@ -520,7 +520,7 @@ static int insert_reads_dev(abb_filter* f, const uint8_t* d_bases, const uint64_
 		ABB_CUDA(cudaEventRecord(f->ev0, f->stream));
 		ABB_CHECK(launch_hash(f, f->k, f->d_care, d_bases, d_offs, f->slot_offs.p, r0, r1, slot_at[c], f->h0.p, f->valid.p,
 		                      f->stream, &f->st.launches));
-		k_count_valid<<<std::min<unsigned>(blocks_for(slots, 256), 148 * 8), 256, 0, f->stream>>>(f->valid.p, slots, f->d_stats + 3);
+		k_count_valid<<<std::min<unsigned>(blocks_for(slots, 256), sm_count() * 8), 256, 0, f->stream>>>(f->valid.p, slots, f->d_stats + 3);
 		f->st.launches += 1;
 		ABB_CUDA(cudaEventRecord(f->ev1, f->stream));
 		if (comm)
@@ -1251,8 +1251,8 @@ int abb_insert_reads_sharded_dev(abb_filter* f, abb_comm* c, const char* d_bases
 	ABB_REQUIRE(f->device == c->device, "filter and communicator live on different devices");
 	ABB_CUDA(cudaSetDevice(f->device));
 	// Policy: the position-sharded insert divides the counter traffic by the world size but every rank still evaluates every
-	// lane and pays a collective per window; measured on B200 it beats one GPU only from 4 ranks on (pass 1 of the bench job:
-	// 2.17 s on 1 GPU, 2.81 s sharded over 2, 1.78 s over 4).  Below ABB_SHARD_MIN_WORLD ranks (default 4) every rank
+	// lane and pays a collective per window, so with few ranks the collectives cost more than the divided traffic saves.
+	// Below ABB_SHARD_MIN_WORLD ranks (default 4) every rank
 	// therefore runs the whole insert itself -- same bytes, no communication -- and only pass 2 is divided.
 	const bool shard = shard_policy(c->world);
 	f->replicated_insert = !shard;
@@ -1342,7 +1342,7 @@ int abb_contains_reads(abb_filter* f, const char* bases, const uint64_t* offsets
 		ABB_CHECK(f->out8.reserve(total));
 		ABB_CHECK(launch_hash(f, f->k, f->d_care, d_bases.p, d_offs.p, f->slot_offs.p, 0, n_reads, 0, f->h0.p, f->valid.p, f->stream, &f->st.launches));
 		const FilterView fv = view_of(f);
-		const unsigned grid = std::min<unsigned>(blocks_for(total, 256), 148 * 16);
+		const unsigned grid = std::min<unsigned>(blocks_for(total, 256), sm_count() * 16);
 		if (f->kind == ABB_COUNTING)
 			k_query_h0<0><<<grid, 256, 0, f->stream>>>(f->h0.p, f->valid.p, total, f->cfg, fv, f->threshold, f->out8.p);
 		else
@@ -1510,7 +1510,7 @@ int abb_filter_popcount(abb_filter* f, uint64_t* nonzero, uint64_t* at_or_above_
 	ABB_CUDA(cudaMemsetAsync(f->d_stats + 4, 0, 2 * sizeof(unsigned long long), f->stream));
 	// bit / cascading: population of the LAST level (the one contains() consults)
 	const uint8_t* p = f->d_data + (uint64_t)(f->levels - 1) * f->bytes_per_level;
-	k_popcount<<<148 * 8, 256, 0, f->stream>>>(p, f->bytes_per_level, f->kind == ABB_COUNTING, f->threshold, f->d_stats + 4);
+	k_popcount<<<sm_count() * 8, 256, 0, f->stream>>>(p, f->bytes_per_level, f->kind == ABB_COUNTING, f->threshold, f->d_stats + 4);
 	f->st.launches += 1;
 	ABB_CUDA(cudaGetLastError());
 	unsigned long long h[2] = { 0, 0 };

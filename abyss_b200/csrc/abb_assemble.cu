@@ -309,9 +309,9 @@ struct WarpCtx {
 				}
 				all &= cov[j] != 0;
 			}
+			__syncwarp(); // cov[] is read back by every lane (walk_read); a vote does not order the stores
 			if (__all_sync(0xffffffffu, all))
 				return;
-			__syncwarp();
 		}
 		// exact fallback: stream the tiles' hashes against a small table of the read's k-mer hashes
 		unsigned cap = 64;
@@ -1487,7 +1487,7 @@ int produce_tiles(abb_assembler* a, uint64_t n_reads, uint64_t n_slots)
 	const unsigned out_cap = (unsigned)std::min<uint64_t>(n_slots / (kMarkerMask + 1) * 2 + 4096, a->marker_set_mask / 2 + 1);
 	ABB_CHECK(a->new_markers.reserve(out_cap));
 	ABB_CUDA(cudaMemsetAsync(a->d_tile_n + 1, 0, 2 * sizeof(unsigned), st));
-	k_find_markers<<<148 * 16, 256, 0, st>>>(a->h0.p, a->valid.p, a->slot_offs.p, n_reads, n_slots, w, f->cfg, a->d_marker_set,
+	k_find_markers<<<sm_count() * 16, 256, 0, st>>>(a->h0.p, a->valid.p, a->slot_offs.p, n_reads, n_slots, w, f->cfg, a->d_marker_set,
 	                                         a->marker_set_mask, a->new_markers.p, a->d_tile_n + 2, out_cap, world, rank);
 	ABB_CUDA(cudaGetLastError());
 	unsigned nm = 0, n0 = 0;
@@ -1504,7 +1504,7 @@ int produce_tiles(abb_assembler* a, uint64_t n_reads, uint64_t n_slots)
 		return ABB_OK;
 	}
 	if (nm) {
-		int sms = 148;
+		int sms = 132;
 		cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, f->device);
 		// persistent warps pulling (marker, orientation, direction) items from a counter: as many CTAs as fit
 		static int tiles_per_sm = 0;
@@ -1541,7 +1541,7 @@ int produce_tiles(abb_assembler* a, uint64_t n_reads, uint64_t n_slots)
 		ABB_CUDA(cudaStreamSynchronize(st));
 		a->st_tiles = nt;
 	}
-	k_link_tiles<<<148 * 8, 256, 0, st>>>(a->d_tiles, (unsigned)a->st_tiles, a->d_tile_tab, a->tile_tab_mask);
+	k_link_tiles<<<sm_count() * 8, 256, 0, st>>>(a->d_tiles, (unsigned)a->st_tiles, a->d_tile_tab, a->tile_tab_mask);
 	ABB_CUDA(cudaGetLastError());
 	a->st_launches += 1;
 	tt.stop();
@@ -1696,7 +1696,7 @@ int stage_contigs(abb_assembler* a, const std::vector<ContigRec>& recs, const Ro
 		ABB_CHECK(h2d(a->seg_beg, seg_beg, st));
 		ABB_CHECK(h2d(a->seg_slot, seg_slot, st));
 		cudaEventRecord(a->ev2[0], st);
-		k_gather<<<std::min<unsigned>(ns, 148 * 16), 256, 0, st>>>(a->recs_sorted.p, a->seg_contig.p, a->seg_beg.p, a->seg_len.p, ns, a->coffs.p,
+		k_gather<<<std::min<unsigned>(ns, sm_count() * 16), 256, 0, st>>>(a->recs_sorted.p, a->seg_contig.p, a->seg_beg.p, a->seg_len.p, ns, a->coffs.p,
 		                                                          a->cseq.p, f->k, a->rt);
 		ABB_CUDA(cudaGetLastError());
 		ABB_CHECK(launch_hash_segments(f->k, f->d_care, a->cseq.p, a->seg_beg.p, a->seg_len.p, a->seg_slot.p, ns, a->ch0.p, a->cvalid.p, st));
@@ -1810,7 +1810,7 @@ int speculate_round(abb_assembler* a, const std::vector<unsigned>& cand, size_t*
 				cudaEventRecord(a->ev2[0], st);
 				ABB_CUDA(cudaMemsetAsync(a->rep_tab.p, 0, tab * sizeof(unsigned long long), st));
 				ABB_CUDA(cudaMemsetAsync(a->rep_flag.p, 0, nc, st));
-				k_repeat_check<<<148 * 8, 256, 0, st>>>(a->recs_sorted.p, nc, a->cslot.p, a->ch0.p, a->rep_tab.p, a->rep_off.p, a->rep_flag.p);
+				k_repeat_check<<<sm_count() * 8, 256, 0, st>>>(a->recs_sorted.p, nc, a->cslot.p, a->ch0.p, a->rep_tab.p, a->rep_off.p, a->rep_flag.p);
 				ABB_CUDA(cudaGetLastError());
 				cudaEventRecord(a->ev2[1], st);
 				++a->st_launches;
@@ -2159,7 +2159,7 @@ static int hash_and_classify(abb_assembler* a, const uint8_t* d_bases, const uin
 	*total_out = total;
 	if (!classify)
 		return ABB_OK;
-	int sms = 148;
+	int sms = 132;
 	cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, f->device);
 	// K3a is pure per read: with a communicator every rank classifies its contiguous slice of the batch and the codes
 	// are all-gathered

@@ -67,6 +67,15 @@ struct DevBuf {
 
 inline unsigned blocks_for(uint64_t n, unsigned threads) { return (unsigned)((n + threads - 1) / threads); }
 
+/** streaming multiprocessors of the current device (132 on an H100 SXM); grid-stride kernels are sized from it */
+inline unsigned sm_count()
+{
+	int dev = 0, n = 0;
+	cudaGetDevice(&dev);
+	cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+	return n > 0 ? (unsigned)n : 132;
+}
+
 // host helpers implemented in abb_api.cu, shared with abb_assemble.cu
 int select_device(int device);
 /** slot_offs[0..n_reads] = exclusive prefix sum of per-read k-mer window counts; *total = sum */

@@ -250,7 +250,7 @@ k_hash_reads(const uint8_t* __restrict__ bases, const uint64_t* __restrict__ off
 	}
 }
 
-// K1 with TMA staging (sm_90+/sm_100a bulk-copy engine).  A CTA of kHashWarps warps takes blocks of kTmaReads consecutive
+// K1 with TMA staging (the Hopper bulk-copy engine).  A CTA of kHashWarps warps takes blocks of kTmaReads consecutive
 // reads; the bytes of a block are contiguous in the batch, so ONE cp.async.bulk (cuda::device::memcpy_async_tx -> UBLKCP)
 // moves them into shared memory and signals an mbarrier; the next block is in flight while the warps hash the current one
 // from shared memory (double buffer; every warp takes kTmaReads / kHashWarps reads of the block, so the two block barriers

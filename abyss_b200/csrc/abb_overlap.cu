@@ -101,7 +101,7 @@ struct abb_overlap {
 
 namespace abb {
 
-static unsigned ovl_grid(uint64_t n) { return (unsigned)std::min<uint64_t>(std::max<uint64_t>(blocks_for(n, 256), 1), 148 * 16); }
+static unsigned ovl_grid(uint64_t n) { return (unsigned)std::min<uint64_t>(std::max<uint64_t>(blocks_for(n, 256), 1), sm_count() * 16); }
 
 /** exclusive sum of n + 1 entries in place (entry n is the total), total copied to the host */
 static int ovl_scan(abb_overlap* h, uint64_t* d, uint64_t n, uint64_t* total)

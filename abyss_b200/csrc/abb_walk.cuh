@@ -647,6 +647,10 @@ ABB_HD bool pathset_insert(Ctx& c, PathSet& ps, uint64_t key, bool* ok)
 		ps.has_zero = true;
 		return fresh;
 	}
+	// every lane must read the slot before any lane writes the key there, or a late lane finds the key and reports a
+	// cycle: extend_dir calls this between Ctx::neighbors_issue and neighbors_finish, where the lanes need not be
+	// converged (with H < 4 some lanes issue no probe and run ahead)
+	c.sync();
 	if ((ps.n + 1) * 2 > ps.cap) { // grow: re-insert everything into a table twice the size
 		PathSet big;
 		if (!pathset_init(c, big, ps.cap * 2)) {

@@ -1,4 +1,4 @@
-// abyss-bloom (B200) -- the `build` command of the reference's abyss-bloom for the ntHash filter
+// abyss-bloom (GPU) -- the `build` command of the reference's abyss-bloom for the ntHash filter
 // family (Bloom/bloom.cc:584-622,625-800): `-t counting` (CountingBloomFilter<uint8_t>, the
 // filter abyss-bloom-dbg loads with -i) and `-t rolling-hash [-l LEVELS]`
 // (HashAgnosticCascadingBloom, last level serialised).  The Konnector filter family (`-t
@@ -79,7 +79,7 @@ int main(int argc, char** argv)
 	if (argc >= 2 && std::string(argv[1]) == "info")
 		return info(argc, argv);
 	if (argc < 2 || std::string(argv[1]) != "build") {
-		std::cerr << PROGRAM ": only the `build' (-t counting | rolling-hash) and `info' commands are implemented on the B200\n";
+		std::cerr << PROGRAM ": only the `build' (-t counting | rolling-hash) and `info' commands are implemented on the GPU\n";
 		usage();
 	}
 	uint64_t bloomSize = 500ULL << 20; // [500M]
@@ -133,7 +133,7 @@ int main(int argc, char** argv)
 		usage();
 	}
 	if (type != "counting" && type != "rolling-hash") {
-		std::cerr << PROGRAM ": `-t " << type << "' is not available on the B200: use 'rolling-hash' or 'counting'\n";
+		std::cerr << PROGRAM ": `-t " << type << "' is not available on the GPU: use 'rolling-hash' or 'counting'\n";
 		usage();
 	}
 	if (argc - optind < 2) {

@@ -1,4 +1,4 @@
-// abyss-bloom-dbg (B200) -- the reference's command line (BloomDBG/bloom-dbg.cc:44-558) over
+// abyss-bloom-dbg (GPU) -- the reference's command line (BloomDBG/bloom-dbg.cc:44-558) over
 // libabyssb200: same options, same AssemblyParams surface, same output, GPU underneath.
 //
 //   abyss-bloom-dbg -b <bloom_size> -H <bloom_hashes> -k <kmer_size> [options] <FASTQ>... > assembly.fasta
@@ -49,9 +49,9 @@ struct AssemblyParams {
 	unsigned trim = UINT_MAX;
 	int verbose = 0;
 	std::string outputPath, tracePath;
-	int device = 0; // B200 extension: --device=N
-	std::string devices; // B200 extension: --devices=LIST, several GPUs (one host thread per GPU)
-	uint64_t batchReads = 4000000; // B200 extension: --batch-reads=N
+	int device = 0; // GPU extension: --device=N
+	std::string devices; // GPU extension: --devices=LIST, several GPUs (one host thread per GPU)
+	uint64_t batchReads = 4000000; // GPU extension: --batch-reads=N
 	bool initialized() const { return bloomSize > 0 && k > 0 && trim != UINT_MAX; }
 	void resetSpacedSeedParams()
 	{
@@ -67,7 +67,7 @@ static const char USAGE_MESSAGE[] =
     "Usage: " PROGRAM " -b <bloom_size> -H <bloom_hashes> -k <kmer_size> \\\n"
     "    [options] <FASTQ> [FASTQ]... > assembly.fasta\n"
     "\n"
-    "Perform a de Bruijn graph assembly of the given FASTQ files on an NVIDIA B200.\n"
+    "Perform a de Bruijn graph assembly of the given FASTQ files on an NVIDIA H100 GPU.\n"
     "\n"
     "Basic Options:\n"
     "\n"
@@ -396,7 +396,7 @@ int main(int argc, char** argv)
 		exit(EXIT_FAILURE);
 	}
 	if (!params.graphPath.empty() && (params.K > 0 || params.qrSeedLen > 0 || !params.spacedSeed.empty())) {
-		std::cerr << PROGRAM ": -g is not supported together with a spaced seed by the B200 implementation\n";
+		std::cerr << PROGRAM ": -g is not supported together with a spaced seed by the GPU implementation\n";
 		exit(EXIT_FAILURE);
 	}
 	/* initGlobals (bloom-dbg.cc:215-233) + MaskedKmer::setMask (BloomDBG/MaskedKmer.h:25-48), once k is known */

@@ -1,4 +1,4 @@
-// AdjList (B200) -- the reference's AdjList command line (AdjList/AdjList.cpp; run by bin/abyss-pe:577 on the unitig
+// AdjList (GPU) -- the reference's AdjList command line (AdjList/AdjList.cpp; run by bin/abyss-pe:577 on the unitig
 // FASTA that abyss-bloom-dbg writes) over libabyssb200: contig ends are hashed, joined and verified on the GPU
 // (abb_overlap_build, csrc/abb_overlap.cu); options, formats and output bytes are the reference's.
 //

@@ -229,7 +229,7 @@ static const char USAGE_MESSAGE[] =
     "Find overlaps of [m,k) bases. Contigs may be read from FILE(s)\n"
     "or standard input. Output is written to standard output.\n"
     "Both the overlaps of exactly k-1 bases and the shorter ones are found\n"
-    "by hash joins on an NVIDIA B200.\n"
+    "by hash joins on an NVIDIA H100 GPU.\n"
     "\n"
     " Options:\n"
     "\n"
@@ -330,7 +330,7 @@ int run(int argc, char** argv, BuildFn build)
 		die = true;
 	}
 	if (singleKmer > 0) {
-		std::cerr << ADJ_PROGRAM ": the paired de Bruijn graph mode (-K) is not supported by the B200 implementation\n";
+		std::cerr << ADJ_PROGRAM ": the paired de Bruijn graph mode (-K) is not supported by the GPU implementation\n";
 		die = true;
 	}
 	if (die) {

@@ -1,4 +1,4 @@
-// reads.h -- host-side FASTA/FASTQ ingestion for the B200 CLI.
+// reads.h -- host-side FASTA/FASTQ ingestion for the GPU CLIs.
 //
 // Mirrors the semantics of the reference reader for the formats the Bloom-DBG stage is fed with
 // (DataLayer/FastaReader.cpp:130-421, FOLD_CASE flag; Common/Uncompress.cpp for .gz/.bz2/.xz):

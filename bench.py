@@ -1,14 +1,16 @@
 #!/usr/bin/env python
-"""bench.py -- the abyss-bloom-dbg hot path on B200 (BASELINE.json metric).
+"""bench.py -- the abyss-bloom-dbg hot path on one H100 (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--reads R]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--reads R] [--dump-outputs DIR]
 
 One "step" = one complete pass of the hot path over the synthetic read set:
     pass 1  ntHash of every k-mer of every read + ordered counting-Bloom insert
     pass 2  classify reads, Bloom-backed unitig extension, ordered replay -> unitig FASTA
-on the workload BASELINE.json's metric is quoted on (configs[1]): 50 M x 150 bp synthetic
-paired reads (187.5 Mbp uniform-random genome, 40x, 0.5 % substitutions), k=64, kc=3, H=4,
--b 8 GiB (7 635 497 472 one-byte counters + 954 437 184 B assembled-k-mer bit filter), 1 x B200.
+on the workload BASELINE.json's metric is quoted on (configs[1]): 32 M x 150 bp synthetic
+paired reads (120 Mbp uniform-random genome, 40x, 0.5 % substitutions), k=64, kc=3, H=4,
+-b 8 GiB (7 635 497 472 one-byte counters + 954 437 184 B assembled-k-mer bit filter), 1 x H100 80 GB.
+Pass 2 takes the whole read set as one batch and needs about 1.1 GB of device memory per million reads on top of the
+reads and the filters, so 32 M reads is what one 80 GB H100 holds with room for the host-buffer arm.
 k-mers/s = (sum over reads of len-k+1) / step time, counted once per input k-mer.
 
 `value`  : reads resident in HBM when the timed region starts (abb_*_dev entry points).
@@ -19,16 +21,17 @@ k-mers/s = (sum over reads of len-k+1) / step time, counted once per input k-mer
            checked here: a mismatch between the e2e and the device-resident arm, or between ranks, fails the run).
 `roofline`: the Bloom-insert kernel (k_insert_windows, the persistent window kernel): algorithmic bytes (64*H B of
            32-byte sectors per inserted k-mer + L/(L-k+1) B of read bases, SURVEY.md section 8d) x the slots its timed
-           launches applied / their summed CUDA-event time, against the measured HBM copy bandwidth in
-           MEASURED_PEAKS.json.  `insert_phase` is the same over the whole insert phase (hash + insert + drains).
+           launches applied / their summed CUDA-event time, against the HBM bandwidth in MEASURED_PEAKS.json where it
+           exists, else the H100 SXM data sheet's 3.35 TB/s.  `insert_phase` is the same over the whole insert phase
+           (hash + insert + drains).
 `cpu_baseline`: the UNMODIFIED reference (oracle/_ref/abyss-bloom-dbg-ref, built by oracle/Makefile) with all host
            threads on a bounded sample (the first S reads of the workload).  Reported: the as-run rate (`value`), the
            start-up cost that depends on -b only (`fixed_s`, 1-read input: zero-filling 8 GiB of filters,
-           contigEndKmers.rehash(2^28), bloom-dbg.h:993), the marginal rate, and -- from profiles/r02_ref_full_run.json --
-           the one FULL 50 M-read run measured on this pool: 626 s with 128 threads = 6.9 M k-mers/s, unitig set
-           identical to this implementation's.  The sample flatters the reference (3x coverage: its extension stage,
-           85 % of the full job's time, hardly runs); see reference_measurement.
+           contigEndKmers.rehash(2^28), bloom-dbg.h:993) and the marginal rate.  The sample flatters the reference
+           (3x coverage: its extension stage, most of the full job's time, hardly runs); see reference_measurement.
+`clocks`  : the GPU's name, power limit and SM clocks during the timed steps.
 `--impl reference` times that reference binary as the step (bounded sample per step).
+`--dump-outputs DIR`: after the timed steps, what the last one computed, as DIR/<name>.npy, see dump_outputs.
 """
 from __future__ import annotations
 
@@ -46,22 +49,22 @@ sys.path.insert(0, ROOT)
 
 K, KC, H, L = 64, 3, 4, 150
 BLOOM_BYTES = 8 << 30
-N_READS = 50_000_000
-GENOME = 187_500_000
+N_READS = 32_000_000
+GENOME = 120_000_000
 ERR = 0.005
 SEED = 2
 REF_BIN = os.path.join(ROOT, "oracle", "_ref", "abyss-bloom-dbg-ref")
 ALG_BYTES_PER_KMER = 64 * H + L / (L - K + 1)  # SURVEY.md section 8(d): 257.7 B
-# dram__bytes_read.sum + dram__bytes_write.sum of one k_insert_windows launch (ncu --set full; profiles/README.md), per
-# k-mer slot applied; None until a capture of this round's kernel exists
-NCU_TRAFFIC_PER_SLOT = 766.6  # 52.93 GB read + 13.76 GB written by the launch that applied 87.0 M slots (profiles/r02_k_insert_windows_final_raw.csv)
+# DRAM bytes read + written per k-mer slot applied by one k_insert_windows launch, from a hardware-counter capture;
+# None: no capture on the H100
+NCU_TRAFFIC_PER_SLOT = None
 
 
 def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return json.load(open(p))["hbm_gbs"], "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 def pass2_rooflines(phases_ms, solid_reads, bases_assembled, peak, world=1):
@@ -90,7 +93,7 @@ def pass2_rooflines(phases_ms, solid_reads, bases_assembled, peak, world=1):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)"""
+    """nvidia-smi clocks / throttle reasons during the timed region, and the card's name and power limit"""
 
     Q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -126,6 +129,15 @@ class ClockSampler:
         reasons = [n for i, n in enumerate(names) if any(s[2 + i].lower().startswith("active") for s in self.samples if len(s) > 2 + i)]
         return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": int(float(self.samples[0][1])), "reasons": reasons}
 
+    def card(self):
+        try:
+            out = subprocess.run(["nvidia-smi", "-i", str(self.index), "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                                 capture_output=True, text=True, timeout=10).stdout.strip()
+            name, power = [x.strip() for x in out.split(",")]
+            return {"gpu": name, "power_limit": power}
+        except Exception:
+            return {"gpu": None, "power_limit": None}
+
 
 def write_sample_fastq(rs, n, path):
     """first n reads of the workload as FASTQ; generated on the GPU when there is one (the numpy generator needs ~8 us/read)"""
@@ -156,11 +168,10 @@ def run_reference(fq, threads, out_fa):
 def reference_measurement(sample, cores, n_runs, warmup=0):
     """The reference on a BOUNDED sample of the workload: its first `sample` reads (same genome, same k / kc / H / -b),
     plus the start-up cost that depends on -b only (1-read input).  No bounded sample is faithful to the full job: this
-    one has ~3x coverage, so almost nothing is solid and the reference's extension stage -- 85 % of its 626 s on the full
-    job -- hardly runs (the sample flatters the reference: 14 M k-mers/s as-run against 6.9 M on the full job); a job of
-    the same SHAPE (2 M reads at 40x of a 7.5 Mbp genome) is the other way round: 195 s = 0.9 M k-mers/s, because 12
-    unitigs give the reference's per-read extension no parallelism.  The full run is recorded in
-    profiles/r02_ref_full_run.json and copied into the line."""
+    one has ~3x coverage, so almost nothing is solid and the reference's extension stage -- most of its time on the full
+    job -- hardly runs (the sample flatters the reference); a job of
+    the same SHAPE (2 M reads at 40x of a 7.5 Mbp genome) is the other way round, because a dozen unitigs give the
+    reference's per-read extension no parallelism."""
     from abyss_b200.synth import ReadSet
     rs = ReadSet(SEED, GENOME, N_READS, L, ERR, paired=True)
     tmp = tempfile.mkdtemp(prefix="abyss_ref_", dir="/dev/shm" if os.path.isdir("/dev/shm") else None)
@@ -179,12 +190,7 @@ def reference_measurement(sample, cores, n_runs, warmup=0):
     os.rmdir(tmp)
     t = sum(times) / len(times)
     kmers = sample * (L - K + 1)
-    m = {"t": t, "fixed_s": fixed, "as_run": kmers / t, "marginal": kmers / max(t - fixed, 1e-3), "kmers": kmers}
-    full = os.path.join(ROOT, "profiles", "r02_ref_full_run.json")
-    if os.path.exists(full):  # one full 50 M-read run of the reference, measured once on this pool (scripts/ref_full_run.py)
-        fr = json.load(open(full))["reference"]
-        m["full_run"] = {"wall_s": fr["wall_s"], "kmers_per_s": fr["kmers_per_s"], "cmd": fr["cmd"], "source": "profiles/r02_ref_full_run.json"}
-    return m
+    return {"t": t, "fixed_s": fixed, "as_run": kmers / t, "marginal": kmers / max(t - fixed, 1e-3), "kmers": kmers}
 
 
 def cpu_baseline_dict(m, cores, sample):
@@ -193,9 +199,7 @@ def cpu_baseline_dict(m, cores, sample):
          "sample": f"first {sample} reads of the workload, abyss-bloom-dbg -j{cores} (unmodified reference), files on tmpfs; "
                    f"{m['t']:.1f} s per run of which {m['fixed_s']:.1f} s do not depend on the reads (1-read run, same -b: zero-filling "
                    "the filters, contigEndKmers.rehash(2^28)); the sample has ~3x coverage, so the reference's extension stage "
-                   "(most of its time on the full job) hardly runs: see full_job_measured"}
-    if "full_run" in m:
-        d["full_job_measured"] = m["full_run"]
+                   "(most of its time on the full job) hardly runs"}
     return d
 
 
@@ -224,6 +228,52 @@ def reference_arm(args, rank, world):
     print(json.dumps(line))
 
 
+DUMP_SAMPLE = 1_000_000  # entries kept of an output larger than this (a fixed, seeded sample): <= 36 MB in all
+
+
+def _sample_index(n, seed):
+    """sorted positions of a fixed sample of an array of n entries (all of them when n <= DUMP_SAMPLE)"""
+    import numpy as np
+    if n <= DUMP_SAMPLE:
+        return np.arange(n, dtype=np.int64)
+    return np.sort(np.random.default_rng(seed).choice(n, DUMP_SAMPLE, replace=False)).astype(np.int64)
+
+
+def dump_outputs(out_dir, asm, filt, counters, n_reads):
+    """What a caller of the timed path receives from the last step, as .npy files: unitigs_{seed_read,length,coverage}
+    (float64, one entry per unitig, in output order), and as float32 the byte arrays unitig_bases (ASCII codes of the
+    unitig sequences concatenated in output order), read_codes (per-read outcome, bloom-dbg.h ReadResult) and counters
+    (the counting filter).  An array longer than DUMP_SAMPLE keeps the entries at DUMP_SAMPLE positions drawn by a
+    numpy default_rng with a fixed seed per array, in increasing order."""
+    import ctypes as C
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+
+    def save(name, values, n, seed, dtype=np.float32):
+        np.save(os.path.join(out_dir, name + ".npy"), np.asarray(values(_sample_index(n, seed)), dtype=dtype))
+
+    recs, n, seqs = asm._last
+    seed_read = np.array([recs[i].seed_read for i in range(n)], dtype=np.float64)
+    length = np.array([recs[i].length for i in range(n)], dtype=np.float64)
+    coverage = np.array([recs[i].coverage for i in range(n)], dtype=np.float64)
+    offset = np.array([recs[i].seq_offset for i in range(n)], dtype=np.int64)
+    save("unitigs_seed_read", lambda i: seed_read[i], n, 11, np.float64)
+    save("unitigs_length", lambda i: length[i], n, 11, np.float64)
+    save("unitigs_coverage", lambda i: coverage[i], n, 11, np.float64)
+    base = C.cast(seqs, C.c_void_p).value if n else 0
+    bases = np.concatenate([np.frombuffer(C.string_at(base + int(o), int(ln)), dtype=np.uint8) for o, ln in zip(offset, length)]) \
+        if n else np.zeros(0, dtype=np.uint8)
+    save("unitig_bases", lambda i: bases[i], bases.size, 12)
+    codes = asm.read_results()
+    save("read_codes", lambda i: codes[i], codes.size, 13)
+
+    class _Dev:  # the filter's device array, seen by torch without a copy to the host
+        __cuda_array_interface__ = {"shape": (counters,), "typestr": "|u1", "data": (filt.device_ptr(), False), "version": 3}
+    dev = torch.as_tensor(_Dev(), device=torch.device("cuda", torch.cuda.current_device()))
+    save("counters", lambda i: dev[torch.from_numpy(i).to(dev.device)].cpu().numpy(), counters, 14)
+
+
 def insert_sharded(world):
     """the library's policy (abb_insert_reads_sharded_dev): below ABB_SHARD_MIN_WORLD ranks (default 4) every rank runs the whole
     insert itself -- the position-sharded insert only beats one GPU from 4 ranks on -- and only pass 2 is divided"""
@@ -245,7 +295,7 @@ def workload_config(args, extra=None):
     c = {"workload": f"{args.reads} x {L} bp synthetic paired reads, {GENOME} bp random genome, err {ERR}, k={K} kc={KC} H={H} -b 8GiB "
                      "(BASELINE.json configs[1])",
          "reads": args.reads, "read_len": L, "k": K, "kc": KC, "num_hashes": H, "bloom_bytes": BLOOM_BYTES,
-         "l2_policy": "inputs (7.5 GB reads) and filters (8.6 GB) far exceed the 126 MB L2; no flush needed",
+         "l2_policy": "inputs (4.8 GB reads) and filters (8.6 GB) far exceed the 50 MB L2; no flush needed",
          "parallelism": parallelism(args.gpus)}
     if extra:
         c.update(extra)
@@ -263,12 +313,19 @@ def main():
     ap.add_argument("--window", type=int, default=0, help="ordered-insert window in k-mer slots (0 = library default)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed to DIR/<name>.npy (float32/float64, seeded samples of the large arrays); "
+                         "--impl ours only.  bench_outputs/ in the repository is git-ignored for this")
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
 
     if args.impl == "reference":
+        if args.dump_outputs:
+            ap.error("--dump-outputs writes what the GPU path computed: it needs --impl ours")
         reference_arm(args, rank, world)
         return
 
@@ -375,8 +432,11 @@ def main():
         timed(1)
     with ClockSampler(local_rank) as clk:
         runs = timed(args.steps)
+    assert len(runs) == args.steps
     ms_step = sum(r[0] for r in runs) / len(runs)
     nk, contigs, ast, ist, cnt = runs[-1][1]
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, asm, filt, counters, rs.n)
     assert nk == n_kmers_expected, (nk, n_kmers_expected)
     total_kmers = nk  # one job, counted once (strong scaling)
     value = total_kmers / (ms_step * 1e-3)
@@ -433,7 +493,9 @@ def main():
                                  "what": "hash + ordered insert + drains" + (" + all-gather of the shards" if sharded else "")}}
 
     cpu = None
-    if not args.no_cpu_baseline and os.path.exists(REF_BIN) and world == 1:
+    if not args.no_cpu_baseline and not os.path.exists(REF_BIN):
+        cpu = {"unavailable": "oracle/_ref/abyss-bloom-dbg-ref not built: build() needs the reference source tree (ABYSS_REFERENCE)"}
+    elif not args.no_cpu_baseline and world == 1:
         cores = os.cpu_count() or 1
         sample = args.ref_reads or 4_000_000
         cpu = cpu_baseline_dict(reference_measurement(min(sample, rs.n), cores, 1), cores, min(sample, rs.n))
@@ -442,7 +504,7 @@ def main():
         "metric": "k-mers/sec (Bloom insert + unitig extend)", "value": value, "unit": "k-mers/s", "n_gpus": world,
         "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms_step, "higher_is_better": True,
         "scaling": "strong", "vs_baseline": None, "dtype": "u8", "data": "synthetic",
-        "config": workload_config(args), "clocks": clk.summary(), "e2e": e2e,
+        "config": workload_config(args), "clocks": {**clk.card(), **clk.summary()}, "e2e": e2e,
         "gpu_launches": int(ist.launches + ast.launches), "roofline": roofline,
         "roofline_pass2": pass2_rooflines({"classify": ast.ms_classify, "tiles": ast.ms_tiles}, int(cnt.solid_reads), int(cnt.bases_assembled),
                                           peak, world),

@@ -1,5 +1,5 @@
 /*
- * abyss_b200.h -- C ABI of libabyssb200.so: the B200 (sm_100a) implementation of the
+ * abyss_b200.h -- C ABI of libabyssb200.so: the H100 (sm_90a) implementation of the
  * abyss-bloom-dbg hot path (ntHash -> Bloom insert -> Bloom-backed unitig extension).
  *
  * The reference (bcgsc/abyss 2.3.10) has no FFI layer: its seam is the duck-typed Bloom filter

@@ -3,7 +3,7 @@
  *
  * Sequential restatement of the reference's hashing and Bloom-filter arithmetic for the
  * abyss-bloom-dbg path.  Written from the reference's behaviour, citing file:line under
- * /root/reference; validated against the compiled reference (tests/test_oracle_*.py).
+ * the reference source tree; validated against the compiled reference (tests/test_oracle_*.py).
  */
 #include "abyss_oracle.h"
 #include <ctype.h>

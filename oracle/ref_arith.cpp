@@ -1,7 +1,7 @@
 // oracle/ref_arith.cpp -- TEST INFRASTRUCTURE ONLY (never linked into the product).
 //
 // Thin command-line harness around the UNMODIFIED reference headers, compiled from
-// /root/reference where they lie (see oracle/Makefile). It exposes the reference's
+// the reference source tree where they lie (see oracle/Makefile). It exposes the reference's
 // arithmetic for this path so that the C restatement (abyss_oracle.c) and the CUDA
 // kernels can be pinned against it:
 //

@@ -1,6 +1,6 @@
-// microbench_random.cu -- what does B200 HBM deliver for the Bloom access pattern?
+// microbench_random.cu -- what does H100 HBM deliver for the Bloom access pattern?
 // Uniform-random 1-byte reads / read-modify-writes over an array much larger than L2, H per "k-mer".
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o microbench_random microbench_random.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o microbench_random microbench_random.cu
 #include <cstdio>
 #include <cstdint>
 #include <cstdlib>

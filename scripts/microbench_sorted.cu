@@ -1,7 +1,7 @@
 // microbench_sorted.cu -- does ordering the Bloom counter accesses by address lift the random-access
-// ceiling of B200 HBM (34 G sector accesses/s, profiles/README.md)?  N byte accesses over a 7.6 GB
+// ceiling of H100 HBM?  N byte accesses over a 7.6 GB
 // array: in random order, fully sorted by address, and sorted only down to bins (random inside a bin).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o microbench_sorted microbench_sorted.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o microbench_sorted microbench_sorted.cu
 #include <cstdio>
 #include <cstdint>
 #include <cstdlib>
@@ -94,7 +94,7 @@ int main(int argc, char** argv) {
 	uint8_t *a, *out; uint64_t *p, *ps, *pb; void* tmp = nullptr; size_t tmp_bytes = 0;
 	const uint64_t nmax = 1ULL << 27;
 	CK(cudaMalloc(&a, m)); CK(cudaMalloc(&out, nmax)); CK(cudaMalloc(&p, nmax * 8)); CK(cudaMalloc(&ps, nmax * 8)); CK(cudaMalloc(&pb, nmax * 8));
-	k_fill<<<148 * 16, 256>>>(a, m); CK(cudaDeviceSynchronize());
+	k_fill<<<132 * 16, 256>>>(a, m); CK(cudaDeviceSynchronize());
 	cub::DeviceRadixSort::SortKeys(nullptr, tmp_bytes, p, ps, (int)nmax);
 	CK(cudaMalloc(&tmp, tmp_bytes));
 	for (int lg = 21; lg <= 27; lg += 2) {

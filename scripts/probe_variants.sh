@@ -1,6 +1,6 @@
 #!/bin/bash
 # GPU probe (not part of the test suite): the bench at 10 M reads under tuning switches; prints hash ms, pass 1 of both arms
-# and the e2e step.  Usage: scripts/probe_variants.sh > gpurun_out/probe.txt
+# and the e2e step.  Usage: scripts/probe_variants.sh > probe.txt
 for v in "ABB_TMA=1 ABB_H2D_OVERLAP=1" "ABB_TMA=0 ABB_H2D_OVERLAP=0"; do
   env $v python bench.py --reads 10000000 --steps 1 --warmup 1 --no-cpu-baseline 2>/dev/null | python -c "
 import json,sys

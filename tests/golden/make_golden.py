@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Regenerate the committed golden fixtures from the UNMODIFIED reference compiled in
-oracle/_ref (see oracle/Makefile; needs /root/reference, i.e. the build container).
+oracle/_ref (see oracle/Makefile; make -C oracle ref REF=<reference source tree>).
 
     make -C oracle ref && python tests/golden/make_golden.py
 

@@ -7,7 +7,7 @@ binary built by oracle/Makefile (oracle/_ref/abyss-bloom-dbg-ref, -j1 is determi
                       in mask_cases.json so that the tests do not depend on the option parser
   mask_<case>.readlog.tsv for the cases marked readlog
 
-Run in the build container only (needs /root/reference through oracle/_ref)."""
+Run in the build container only (needs the reference binaries in oracle/_ref: make -C oracle ref REF=...)."""
 import gzip
 import json
 import os

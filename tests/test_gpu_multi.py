@@ -1,4 +1,4 @@
-"""Multi-GPU tests of the exact position-sharded pass 1 (run under `gpurun --gpus 2` or more; skipped with one device).
+"""Multi-GPU tests of the exact position-sharded pass 1 (they need 2 or more GPUs and skip with one).
 At every world size the counters must be the sequential -j1 array bit for bit (sha256 of the reference's
 `abyss-bloom build -t counting` output, tests/golden/e2e_cases.json) and the unitig FASTA byte-identical to the
 reference's (tests/golden/*.fa) -- the same goldens the single-GPU tests use."""

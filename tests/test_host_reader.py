@@ -10,6 +10,8 @@ import subprocess
 
 import pytest
 
+import ref_golden
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
@@ -89,27 +91,30 @@ def test_stream_quality_options(exe, tmp_path):
         assert got == want
 
 
-REF_ARITH = os.path.join(ROOT, "oracle", "_ref", "ref_arith")
-
-
-@pytest.mark.skipif(not os.path.exists(REF_ARITH), reason="oracle/_ref not built (needs /root/reference)")
-def test_reader_equals_reference_reader(exe, tmp_path):
-    # the UNMODIFIED reference reader (DataLayer/FastaReader.cpp through oracle/_ref/ref_arith reads dump):
-    # ids (Casava suffix), chastity filter, masked-end trimming, case folding, multi-line FASTA, CRLF, gz
-    files = {"a.fq": fastq(2000, 11), "b.fq": fastq(1000, 12, crlf=True, casava=True), "c.fa": fasta(500, 13)}
+def write_files(d, files):
     paths = []
     for name, text in files.items():
-        p = tmp_path / name
-        p.write_text(text, newline="")
-        paths.append(str(p))
-    gz = tmp_path / "g.fq.gz"
+        p = os.path.join(d, name)
+        with open(p, "w", newline="") as f:
+            f.write(text)
+        paths.append(p)
+    return paths
+
+
+def write_reader_files(d):
+    paths = write_files(d, {"a.fq": fastq(2000, 11), "b.fq": fastq(1000, 12, crlf=True, casava=True), "c.fa": fasta(500, 13)})
+    gz = os.path.join(d, "g.fq.gz")
     with gzip.open(gz, "wt", newline="") as f:
         f.write(fastq(300, 14))
-    paths.append(str(gz))
-    ref = subprocess.run([REF_ARITH, "reads", "dump", *paths], capture_output=True, text=True)
-    assert ref.returncode == 0, ref.stderr
+    return paths + [gz]
+
+
+def test_reader_equals_reference_reader(exe, tmp_path):
+    # the UNMODIFIED reference reader (DataLayer/FastaReader.cpp, `reads dump` of oracle/ref_arith.cpp):
+    # ids (Casava suffix), chastity filter, masked-end trimming, case folding, multi-line FASTA, CRLF, gz
+    paths = write_reader_files(str(tmp_path))
     got, _ = run(exe, "stream", 3, 500, 4096, *paths)
-    assert got == ref.stdout
+    assert ref_golden.matches(got, ref_golden.load("reader"))
 
 
 def test_long_records(exe, tmp_path):
@@ -199,29 +204,33 @@ def qseq_text(n, seed, export=False):
     return "\n".join(out) + "\n"
 
 
-@pytest.mark.skipif(not os.path.exists(REF_ARITH), reason="oracle/_ref not built (needs /root/reference)")
-@pytest.mark.parametrize("opts", [{}, {"Q": "20"}, {"MASKQ": "15"}, {"NO_CHASTITY": "1"}, {"Q": "10", "QOFF": "64"}, {"MASKQ": "12", "QOFF": "33"},
-                                  {"NO_TRIM_MASKED": "1"}])
+READER_OPTS = [{}, {"Q": "20"}, {"MASKQ": "15"}, {"NO_CHASTITY": "1"}, {"Q": "10", "QOFF": "64"}, {"MASKQ": "12", "QOFF": "33"},
+               {"NO_TRIM_MASKED": "1"}]
+
+
+def opts_key(opts):
+    return ",".join(f"{k}={v}" for k, v in sorted(opts.items())) or "default"
+
+
+def write_sam_qseq_files(d):
+    return write_files(d, {"a.sam": sam_text(800, 21), "b_qseq.txt": qseq_text(600, 22), "c_export.txt": qseq_text(400, 23, export=True),
+                           "d.fq": fastq(500, 24, casava=True), "e.fa": fasta(200, 25)})
+
+
+@pytest.mark.parametrize("opts", READER_OPTS)
 def test_sam_qseq_export_equal_reference_reader(exe, tmp_path, opts):
     # the record formats of DataLayer/FastaReader.cpp:270-352 next to FASTQ, with the reader options of the command line
     # (-q, -Q, --illumina-quality / --standard-quality, --no-chastity, --no-trim-masked), against the UNMODIFIED reference reader
-    files = {"a.sam": sam_text(800, 21), "b_qseq.txt": qseq_text(600, 22), "c_export.txt": qseq_text(400, 23, export=True),
-             "d.fq": fastq(500, 24, casava=True), "e.fa": fasta(200, 25)}
-    paths = []
-    for name, text in files.items():
-        p = tmp_path / name
-        p.write_text(text, newline="")
-        paths.append(str(p))
-    ref = subprocess.run([REF_ARITH, "reads", "dump", *paths], capture_output=True, text=True, env=dict(os.environ, **{"REF_" + k: v for k, v in opts.items()}))
-    assert ref.returncode == 0, ref.stderr
+    paths = write_sam_qseq_files(str(tmp_path))
+    want = ref_golden.load("reader_formats")[opts_key(opts)]
     env = {"READER_" + k: v for k, v in opts.items()}
     serial, _ = run(exe, "serial", *paths, env=env)
-    assert serial == ref.stdout
+    assert ref_golden.matches(serial, want)
     got, _ = run(exe, "stream", 3, 250, 4096, *paths, env=env)
-    assert got == ref.stdout
+    assert got == serial
     got, _ = run(exe, "stream", 3, 250, 4096, *paths, env=dict(env, ABB_NO_MMAP="1"))
-    assert got == ref.stdout
-    assert ref.stdout.count("\n") > 1500
+    assert got == serial
+    assert serial.count("\n") > 1500
 
 
 @pytest.mark.parametrize("mapped", [True, False])

@@ -15,7 +15,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libabyssb200.so")
 
 ABB_OK, ABB_EINVAL, ABB_ENODEV, ABB_ECUDA, ABB_ENOMEM, ABB_ESTATE = 0, -1, -2, -3, -4, -5
-COUNTING, BIT, CASCADING = 0, 1, 2
+COUNTING, BIT, CASCADING, KONNECTOR = 0, 1, 2, 3
 
 
 class AbbError(RuntimeError):
@@ -84,6 +84,10 @@ SIGNATURES = {
     "abb_device_count": (C.c_int, []),
     "abb_filter_create": (C.c_int, [C.POINTER(_vp), C.c_int, C.c_uint64, C.c_uint, C.c_uint, C.c_uint, C.c_char_p, C.c_int]),
     "abb_filter_destroy": (C.c_int, [_vp]),
+    "abb_konnector_create": (C.c_int, [C.POINTER(_vp), C.c_uint64, C.c_uint, C.c_uint, C.c_uint64, C.c_uint64, C.c_uint64, C.c_int]),
+    "abb_filter_read_bits": (C.c_int, [_vp, C.c_int, _vp, C.c_uint64, C.c_uint64, C.c_int]),
+    "abb_filter_compare": (C.c_int, [_vp, _vp, _u64p]),
+    "abb_filter_level_popcount": (C.c_int, [_vp, C.c_int, _u64p]),
     "abb_filter_kmer_size": (C.c_uint, [_vp]),
     "abb_filter_hash_num": (C.c_uint, [_vp]),
     "abb_filter_size": (C.c_uint64, [_vp]),
@@ -243,13 +247,43 @@ class Filter:
     kind COUNTING  ~ CountingBloomFilter<uint8_t>(size, H, k, threshold)  (CountingBloomFilter.hpp:31-50)
     kind BIT       ~ BloomFilter(size_bits, H, k)                          (BloomFilter.hpp:64-74)
     kind CASCADING ~ HashAgnosticCascadingBloom(size_bits, H, levels, k)   (HashAgnosticCascadingBloom.h:43-55)
+    kind KONNECTOR ~ Konnector::BloomFilter / CascadingBloomFilter[Window](full_bits, levels, seed)  (Bloom/BloomFilter.h)
     """
 
-    def __init__(self, kind: int, size: int, num_hashes: int, k: int, arg: int = 0, mask: str = "", device: int = 0):
+    def __init__(self, kind: int, size: int, num_hashes: int, k: int, arg: int = 0, mask: str = "", device: int = 0, _handle=None):
         self._lib = load()
         self._h = _vp()
-        check(self._lib.abb_filter_create(C.byref(self._h), kind, size, num_hashes, k, arg, mask.encode(), device))
+        if _handle is not None:
+            self._h = _handle
+        else:
+            check(self._lib.abb_filter_create(C.byref(self._h), kind, size, num_hashes, k, arg, mask.encode(), device))
         self.kind = kind
+
+    @classmethod
+    def konnector(cls, full_bits, k, levels=1, seed=0, start_bit=0, end_bit=None, device=0):
+        """`abyss-bloom build -t konnector`: `levels` levels holding bits [start_bit, end_bit] of a filter of full_bits bits"""
+        lib = load()
+        h = _vp()
+        check(lib.abb_konnector_create(C.byref(h), full_bits, k, levels, seed, start_bit, full_bits - 1 if end_bit is None else end_bit,
+                                       device))
+        return cls(KONNECTOR, 0, 1, k, _handle=h)
+
+    def read_bits(self, data: np.ndarray, bits: int, bit_offset: int = 0, op: int = 0, level: int = -1):
+        """readBits (Common/BitUtil.h): op 0 overwrite, 1 or, 2 and"""
+        data = np.ascontiguousarray(data, dtype=np.uint8)
+        assert data.size * 8 >= bits
+        check(self._lib.abb_filter_read_bits(self._h, level, _ptr(data), bits, bit_offset, op))
+
+    def compare(self, other: "Filter") -> tuple[int, int, int, int]:
+        """the 1/1, 1/0, 0/1, 0/0 bit counts of `abyss-bloom compare`"""
+        n = (C.c_uint64 * 4)()
+        check(self._lib.abb_filter_compare(self._h, other._h, n))
+        return tuple(int(x) for x in n)
+
+    def level_popcount(self, level: int = -1) -> int:
+        n = C.c_uint64(0)
+        check(self._lib.abb_filter_level_popcount(self._h, level, C.byref(n)))
+        return n.value
 
     @classmethod
     def counting(cls, counters, num_hashes, k, threshold=0, mask="", device=0):

@@ -788,11 +788,14 @@ int abb_device_count(void)
 	return n;
 }
 
+static int alloc_filter(abb_filter* f, abb_filter** out);
+
 int abb_filter_create(abb_filter** out, int kind, uint64_t size, unsigned num_hashes, unsigned k, unsigned arg,
                       const char* mask, int device)
 {
 	ABB_REQUIRE(out != nullptr, "abb_filter_create: out is NULL");
 	*out = nullptr;
+	ABB_REQUIRE(kind != ABB_KONNECTOR, "Konnector filters are created with abb_konnector_create");
 	ABB_REQUIRE(kind == ABB_COUNTING || kind == ABB_BIT || kind == ABB_CASCADING, "unknown filter kind %d", kind);
 	ABB_REQUIRE(num_hashes >= 1 && num_hashes <= kMaxHashes, "number of hash functions must be in 1..%u (MAX_HASHES)", kMaxHashes);
 	ABB_REQUIRE(k >= 1 && k <= kMaxK, "k-mer size must be in 1..%u (MAX_KMER)", kMaxK);
@@ -842,6 +845,13 @@ int abb_filter_create(abb_filter** out, int kind, uint64_t size, unsigned num_ha
 	f->cfg.mod = make_fastmod(size);
 	for (unsigned i = 0; i < kMaxHashes; ++i)
 		f->cfg.mult[i] = (uint64_t)i ^ ((uint64_t)k * kMultiSeed); // nthash.hpp:339
+	return alloc_filter(f, out);
+}
+
+/** the device side of a filter whose geometry is set: stream, events, the zeroed levels, control words.  Frees f on failure. */
+static int alloc_filter(abb_filter* f, abb_filter** out)
+{
+	const unsigned k = f->k, levels = f->levels;
 	auto fail = [&](int rc) {
 		abb_filter_destroy(f);
 		return rc;
@@ -875,6 +885,35 @@ int abb_filter_create(abb_filter** out, int kind, uint64_t size, unsigned num_ha
 #undef ABB_TRY
 	*out = f;
 	return ABB_OK;
+}
+
+int abb_konnector_create(abb_filter** out, uint64_t full_bits, unsigned k, unsigned levels, uint64_t hash_seed, uint64_t start_bit,
+                         uint64_t end_bit, int device)
+{
+	ABB_REQUIRE(out != nullptr, "abb_konnector_create: out is NULL");
+	*out = nullptr;
+	ABB_REQUIRE(k >= 1 && k <= kMaxK, "k-mer size must be in 1..%u (MAX_KMER)", kMaxK);
+	ABB_REQUIRE(full_bits >= 2, "a Konnector filter needs at least 2 bits");
+	ABB_REQUIRE(start_bit <= end_bit && end_bit < full_bits, "window [%llu, %llu] is not inside a filter of %llu bits",
+	            (unsigned long long)start_bit, (unsigned long long)end_bit, (unsigned long long)full_bits);
+	ABB_REQUIRE(levels >= 1 && levels <= 255, "a Konnector filter needs 1..255 levels");
+	ABB_CHECK(select_device(device));
+	abb_filter* f = new (std::nothrow) abb_filter();
+	if (!f) {
+		set_error("out of host memory");
+		return ABB_ENOMEM;
+	}
+	f->device = device;
+	f->kind = ABB_KONNECTOR;
+	f->size = end_bit - start_bit + 1;
+	f->bytes_per_level = (f->size + 7) / 8;
+	f->H = 1;
+	f->k = k;
+	f->levels = levels;
+	f->kon_full = full_bits;
+	f->kon_start = start_bit;
+	f->kon_seed = hash_seed;
+	return alloc_filter(f, out);
 }
 
 int abb_filter_destroy(abb_filter* f)
@@ -975,6 +1014,8 @@ int abb_insert_reads_dev(abb_filter* f, const char* d_bases, const uint64_t* d_o
 	ABB_REQUIRE(f, "NULL filter");
 	ABB_REQUIRE(n_reads == 0 || (d_bases && d_offsets), "NULL read buffers");
 	ABB_CUDA(cudaSetDevice(f->device));
+	if (f->kind == ABB_KONNECTOR)
+		return kon_insert_reads_dev(f, (const uint8_t*)d_bases, d_offsets, n_reads, n_kmers_out);
 	return insert_reads_dev(f, (const uint8_t*)d_bases, d_offsets, n_reads, n_kmers_out);
 }
 
@@ -993,6 +1034,10 @@ int abb_insert_reads(abb_filter* f, const char* bases, const uint64_t* offsets, 
 	ABB_CHECK(f->offs.reserve(n_reads + 1));
 	ABB_CUDA(cudaMemcpyAsync(f->offs.p, offsets, (n_reads + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, f->stream));
 	f->resident_reads = n_reads;
+	if (f->kind == ABB_KONNECTOR) {
+		ABB_CUDA(cudaMemcpyAsync(f->bases.p, bases, n_bases, cudaMemcpyHostToDevice, f->stream));
+		return kon_insert_reads_dev(f, f->bases.p, f->offs.p, n_reads, n_kmers_out);
+	}
 	// The bases travel in pieces on a second stream; chunk c of the insert only waits for the pieces that hold its reads, so
 	// the copy of the rest hides behind the hashing and inserting of the earlier chunks (with pinned host memory; a pageable
 	// buffer makes cudaMemcpyAsync synchronous and the order is simply copy, then insert).  ABB_H2D_OVERLAP=0: one copy up front.
@@ -1050,6 +1095,7 @@ int abb_insert_reads_sharded(abb_filter* f, abb_comm* c, const char* bases, cons
                              uint64_t* n_kmers_out)
 {
 	ABB_REQUIRE(f && c, "NULL argument");
+	ABB_REQUIRE_NTHASH(f);
 	if (!shard_policy(c->world)) { // replicated insert: the single-GPU host path, with its copy hidden behind the insert
 		ABB_REQUIRE(f->kind == ABB_COUNTING, "the sharded insert is implemented for counting filters");
 		ABB_REQUIRE(f->device == c->device, "filter and communicator live on different devices");
@@ -1085,6 +1131,7 @@ int abb_filter_resident_reads(abb_filter* f, const char** d_bases, const uint64_
 int abb_insert_hashes(abb_filter* f, const uint64_t* hashes, uint64_t n)
 {
 	ABB_REQUIRE(f, "NULL filter");
+	ABB_REQUIRE_NTHASH(f);
 	if (n == 0)
 		return ABB_OK;
 	ABB_REQUIRE(hashes, "NULL hashes");
@@ -1100,6 +1147,7 @@ int abb_insert_hashes(abb_filter* f, const uint64_t* hashes, uint64_t n)
 int abb_insert_h0_dev(abb_filter* f, const uint64_t* d_h0, uint64_t n)
 {
 	ABB_REQUIRE(f, "NULL filter");
+	ABB_REQUIRE_NTHASH(f);
 	if (n == 0)
 		return ABB_OK;
 	ABB_REQUIRE(d_h0, "NULL hashes");
@@ -1115,6 +1163,7 @@ int abb_hash_reads_dev(abb_filter* f, const char* d_bases, const uint64_t* d_off
                        uint8_t* d_valid, uint64_t capacity, uint64_t* n_slots_out)
 {
 	ABB_REQUIRE(f, "NULL filter");
+	ABB_REQUIRE_NTHASH(f);
 	if (n_slots_out)
 		*n_slots_out = 0;
 	if (n_reads == 0)
@@ -1189,6 +1238,7 @@ int abb_comm_world(const abb_comm* c) { return c ? c->world : 1; }
 int abb_filter_allgather(abb_filter* f, abb_comm* c)
 {
 	ABB_REQUIRE(f && c, "NULL argument");
+	ABB_REQUIRE_NTHASH(f);
 	ABB_REQUIRE(f->levels == 1, "only single-level filters are sharded");
 	ABB_CUDA(cudaSetDevice(f->device));
 	if (c->world == 1 || f->replicated_insert)
@@ -1246,6 +1296,7 @@ int abb_insert_reads_sharded_dev(abb_filter* f, abb_comm* c, const char* d_bases
                                  int finalize, uint64_t* n_kmers_out)
 {
 	ABB_REQUIRE(f && c, "NULL argument");
+	ABB_REQUIRE_NTHASH(f);
 	ABB_REQUIRE(f->kind == ABB_COUNTING, "the sharded insert is implemented for counting filters");
 	ABB_REQUIRE(n_reads == 0 || (d_bases && d_offsets), "NULL read buffers");
 	ABB_REQUIRE(f->device == c->device, "filter and communicator live on different devices");
@@ -1278,6 +1329,7 @@ void* abb_filter_device_ptr(abb_filter* f, int level)
 static int query_hashes(abb_filter* f, const uint64_t* hashes, uint64_t n, uint8_t* out, bool want_min)
 {
 	ABB_REQUIRE(f, "NULL filter");
+	ABB_REQUIRE_NTHASH(f);
 	if (n == 0)
 		return ABB_OK;
 	ABB_REQUIRE(hashes && out, "NULL buffer");
@@ -1337,18 +1389,22 @@ int abb_contains_reads(abb_filter* f, const char* bases, const uint64_t* offsets
 		if (total == 0 || (!out_flag && !out_valid))
 			return ABB_OK;
 		ABB_REQUIRE(capacity >= total, "output buffers hold %llu slots, %llu needed", (unsigned long long)capacity, (unsigned long long)total);
-		ABB_CHECK(f->h0.reserve(total));
 		ABB_CHECK(f->valid.reserve(total));
 		ABB_CHECK(f->out8.reserve(total));
-		ABB_CHECK(launch_hash(f, f->k, f->d_care, d_bases.p, d_offs.p, f->slot_offs.p, 0, n_reads, 0, f->h0.p, f->valid.p, f->stream, &f->st.launches));
-		const FilterView fv = view_of(f);
-		const unsigned grid = std::min<unsigned>(blocks_for(total, 256), sm_count() * 16);
-		if (f->kind == ABB_COUNTING)
-			k_query_h0<0><<<grid, 256, 0, f->stream>>>(f->h0.p, f->valid.p, total, f->cfg, fv, f->threshold, f->out8.p);
-		else
-			k_query_h0<1><<<grid, 256, 0, f->stream>>>(f->h0.p, f->valid.p, total, f->cfg, fv, 0, f->out8.p);
-		f->st.launches += 1;
-		ABB_CUDA(cudaGetLastError());
+		if (f->kind == ABB_KONNECTOR)
+			ABB_CHECK(kon_query_slots(f, d_bases.p, d_offs.p, n_reads, total));
+		else {
+			ABB_CHECK(f->h0.reserve(total));
+			ABB_CHECK(launch_hash(f, f->k, f->d_care, d_bases.p, d_offs.p, f->slot_offs.p, 0, n_reads, 0, f->h0.p, f->valid.p, f->stream, &f->st.launches));
+			const FilterView fv = view_of(f);
+			const unsigned grid = std::min<unsigned>(blocks_for(total, 256), sm_count() * 16);
+			if (f->kind == ABB_COUNTING)
+				k_query_h0<0><<<grid, 256, 0, f->stream>>>(f->h0.p, f->valid.p, total, f->cfg, fv, f->threshold, f->out8.p);
+			else
+				k_query_h0<1><<<grid, 256, 0, f->stream>>>(f->h0.p, f->valid.p, total, f->cfg, fv, 0, f->out8.p);
+			f->st.launches += 1;
+			ABB_CUDA(cudaGetLastError());
+		}
 		if (out_flag)
 			ABB_CUDA(cudaMemcpyAsync(out_flag, f->out8.p, total, cudaMemcpyDeviceToHost, f->stream));
 		if (out_valid)
@@ -1364,6 +1420,7 @@ int abb_contains_reads(abb_filter* f, const char* bases, const uint64_t* offsets
 int abb_successors(abb_filter* f, const char* kmers, uint64_t n, unsigned max_chain, abb_succ_info* out, unsigned* out_len, uint64_t* self_hash)
 {
 	ABB_REQUIRE(f, "NULL filter");
+	ABB_REQUIRE_NTHASH(f);
 	if (n == 0)
 		return ABB_OK;
 	ABB_REQUIRE(kmers && out && out_len && self_hash, "NULL buffer");
@@ -1506,6 +1563,15 @@ int abb_filter_clear(abb_filter* f)
 int abb_filter_popcount(abb_filter* f, uint64_t* nonzero, uint64_t* at_or_above_threshold)
 {
 	ABB_REQUIRE(f, "NULL filter");
+	if (f->kind == ABB_KONNECTOR) { // its levels need not start on a 16-byte boundary
+		uint64_t n = 0;
+		ABB_CHECK(abb_filter_level_popcount(f, -1, &n));
+		if (nonzero)
+			*nonzero = n;
+		if (at_or_above_threshold)
+			*at_or_above_threshold = n;
+		return ABB_OK;
+	}
 	ABB_CUDA(cudaSetDevice(f->device));
 	ABB_CUDA(cudaMemsetAsync(f->d_stats + 4, 0, 2 * sizeof(unsigned long long), f->stream));
 	// bit / cascading: population of the LAST level (the one contains() consults)

@@ -38,6 +38,15 @@ void set_error(const char* fmt, ...);
 		}                              \
 	} while (0)
 
+/** entry points of the ntHash filter kinds (hash arrays, spaced seeds, the sharded insert, graph queries) */
+#define ABB_REQUIRE_NTHASH(f)                                                                       \
+	do {                                                                                            \
+		if ((f)->kind == ABB_KONNECTOR) {                                                           \
+			abb::set_error("%s: not available for Konnector (-t konnector) filters", __func__);     \
+			return ABB_ESTATE;                                                                      \
+		}                                                                                           \
+	} while (0)
+
 /** growable device buffer */
 template <typename T>
 struct DevBuf {
@@ -92,6 +101,10 @@ int launch_hash(abb_filter* f, unsigned k, const uint8_t* d_care, const uint8_t*
                 cudaStream_t stream, uint64_t* launches);
 int launch_hash_segments(unsigned k, const uint8_t* d_care, const uint8_t* d_bases, const uint64_t* d_seg_beg, const unsigned* d_seg_len,
                          const uint64_t* d_seg_slot, uint64_t n_segs, uint64_t* d_h0, uint8_t* d_valid, cudaStream_t stream);
+// abb_konnector.cu: the ABB_KONNECTOR paths of abb_insert_reads(_dev) and abb_contains_reads
+int kon_insert_reads_dev(abb_filter* f, const uint8_t* d_bases, const uint64_t* d_offs, uint64_t n_reads, uint64_t* n_kmers_out);
+/** membership of the last level and validity of every window slot (f->slot_offs already computed) into f->out8 / f->valid */
+int kon_query_slots(abb_filter* f, const uint8_t* d_bases, const uint64_t* d_offs, uint64_t n_reads, uint64_t n_slots);
 }
 
 /** The filter handle (opaque in the C ABI). */
@@ -101,6 +114,7 @@ struct abb_filter {
 	uint64_t size = 0;            // counters, or bits per level
 	uint64_t bytes_per_level = 0; // bytes of one level
 	unsigned H = 0, k = 0, threshold = 0, levels = 1;
+	uint64_t kon_full = 0, kon_start = 0, kon_seed = 0; // ABB_KONNECTOR: filter size in bits, first bit held, hash seed
 	std::string mask;
 	uint8_t* d_care = nullptr; // k bytes (mask == '1'), only with a spaced seed
 	uint8_t* d_data = nullptr;

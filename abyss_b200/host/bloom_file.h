@@ -5,8 +5,10 @@
 // Key order follows what the reference writes (cpptoml unordered_map iteration order under
 // libstdc++), so files are byte-identical; loaders parse by key.
 #pragma once
+#include <cerrno>
 #include <cstdint>
 #include <cstdlib>
+#include <cstring>
 #include <fstream>
 #include <iostream>
 #include <map>
@@ -125,6 +127,81 @@ inline void write_bit_bloom(std::ostream& out, uint64_t sizeBits, unsigned hashN
 	    << "\tKmerSize = " << kmerSize << "\n"
 	    << "[HeaderEnd]\n";
 	out.write(reinterpret_cast<const char*>(raw.data()), (std::streamsize)raw.size());
+}
+
+/** The Konnector filter file (Bloom/Bloom.h:136-191): a text header "5\n{k}\n{full}\t{start}\t{end}\n{seed}\n" and the bits
+ *  [start, end] of a filter of `full` bits, (end - start + 1 + 7) / 8 bytes, bit i in byte i/8 under mask 0x80 >> i%8. */
+struct KonnectorHeader {
+	unsigned version = 5, k = 0;
+	uint64_t full = 0, start = 0, end = 0, seed = 0;
+	uint64_t bits() const { return end - start + 1; }
+	uint64_t bytes() const { return (bits() + 7) / 8; }
+};
+
+/** true if the first line of the file is a Konnector header ("5"), false for anything else (the BTL formats) */
+inline bool is_konnector_bloom(const std::string& path)
+{
+	std::ifstream in(path, std::ios::binary);
+	std::string line;
+	return in && std::getline(in, line) && !line.empty() && line.find_first_not_of("0123456789") == std::string::npos;
+}
+
+/** Bloom::readHeader with its messages and exits; k = 0 skips the k check */
+inline KonnectorHeader read_konnector_header(std::istream& in, unsigned k)
+{
+	KonnectorHeader h;
+	char c1 = 0, c2 = 0, c3 = 0, c4 = 0, c5 = 0;
+	in >> h.version;
+	in.get(c1);
+	if (h.version != 5) {
+		std::cerr << "error: bloom filter version (`" << h.version << "'), does not match version required by this program (`5').\n";
+		exit(EXIT_FAILURE);
+	}
+	in >> h.k;
+	in.get(c2);
+	if (k != 0 && h.k != k) {
+		std::cerr << "error: this program must be run with the same kmer size as the bloom filter being loaded (k=" << h.k << ").\n";
+		exit(EXIT_FAILURE);
+	}
+	in >> h.full;
+	in.get(c3);
+	in >> h.start;
+	in.get(c4);
+	in >> h.end;
+	in.get(c5);
+	in >> h.seed;
+	char c6 = 0;
+	in.get(c6);
+	if (!in || c1 != '\n' || c2 != '\n' || c3 != '\t' || c4 != '\t' || c5 != '\n' || c6 != '\n' || h.start >= h.full || h.end >= h.full ||
+	    h.start > h.end) {
+		std::cerr << "error: malformed Konnector Bloom filter header\n";
+		exit(EXIT_FAILURE);
+	}
+	return h;
+}
+
+/** the header and the raw bytes of a Konnector filter file */
+inline KonnectorHeader read_konnector_bloom(const std::string& path, unsigned k, std::vector<uint8_t>& raw)
+{
+	std::ifstream in(path, std::ios::binary);
+	if (!in) {
+		std::cerr << "error: `" << path << "': " << strerror(errno) << "\n";
+		exit(EXIT_FAILURE);
+	}
+	KonnectorHeader h = read_konnector_header(in, k);
+	raw.resize(h.bytes());
+	in.read(reinterpret_cast<char*>(raw.data()), (std::streamsize)raw.size());
+	if (!in) {
+		std::cerr << "error: `" << path << "': truncated filter\n";
+		exit(EXIT_FAILURE);
+	}
+	return h;
+}
+
+inline void write_konnector_bloom(std::ostream& out, const KonnectorHeader& h, const uint8_t* raw)
+{
+	out << 5 << '\n' << h.k << '\n' << h.full << '\t' << h.start << '\t' << h.end << '\n' << h.seed << '\n';
+	out.write(reinterpret_cast<const char*>(raw), (std::streamsize)h.bytes());
 }
 
 } // namespace host

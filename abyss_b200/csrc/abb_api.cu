@@ -65,7 +65,7 @@ int select_device(int device)
 static FilterView view_of(const abb_filter* f)
 {
 	FilterView v;
-	v.data = f->d_data;
+	v.data = f->d_data.p;
 	v.level_stride = f->bytes_per_level;
 	v.levels = f->levels;
 	return v;
@@ -96,37 +96,36 @@ static unsigned age_windows_for(uint64_t window)
 static int ensure_workspace(abb_filter* f)
 {
 	const uint64_t want_entries = map_entries_for(f->size, f->map_log2 ? f->map_log2 : 25);
-	if (f->d_carry && f->ws_window == f->window && f->ws_H == f->H && f->map_entries == want_entries)
+	if (f->d_carry.p && f->ws_window == f->window && f->ws_H == f->H && f->map_entries == want_entries)
 		return ABB_OK;
-	cudaFree(f->d_map[0]); // one allocation holds both maps (one L2 access-policy window covers them)
-	for (int i = 0; i < 2; ++i) {
-		cudaFree(f->d_tags2[i]);
-		f->d_tags2[i] = nullptr;
-	}
+	// the old workspace is freed before the new one is allocated (peak memory), and it counts as valid again only once
+	// every piece has been allocated
+	f->ws_window = 0;
 	f->d_map[0] = f->d_map[1] = f->d_map[2] = nullptr;
-	cudaFree(f->d_carry);
-	cudaFree(f->d_slotbits);
-	f->d_carry = nullptr;
-	f->d_slotbits = nullptr;
-	f->map_entries = want_entries;
-	const size_t map_bytes = std::max<size_t>(f->map_entries / 4, 256);
+	f->maps.reset();
+	f->d_tags2[0].reset();
+	f->d_tags2[1].reset();
+	f->d_carry.reset();
+	f->d_slotbits.reset();
+	const size_t map_words = std::max<size_t>(want_entries / 4, 256) / sizeof(unsigned);
 	// at most kCarryLanes carried slots reserve H positions each; load factor <= 1/8.  Only a prefix sized to the
 	// carried slots of a window is in use (tag_mask_for)
 	f->tag_slots = next_pow2(8ULL * kCarryLanes * f->H);
-	ABB_CUDA(cudaMalloc((void**)&f->d_map[0], 3 * map_bytes));
-	ABB_CUDA(cudaMemsetAsync(f->d_map[0], 0, 3 * map_bytes, f->stream));
-	f->d_map[1] = f->d_map[0] + map_bytes / sizeof(unsigned);
-	f->d_map[2] = f->d_map[1] + map_bytes / sizeof(unsigned);
-	for (int i = 0; i < 2; ++i) {
-		ABB_CUDA(cudaMalloc((void**)&f->d_tags2[i], f->tag_slots * sizeof(unsigned long long)));
-		ABB_CUDA(cudaMemsetAsync(f->d_tags2[i], 0, f->tag_slots * sizeof(unsigned long long), f->stream));
+	ABB_CHECK(f->maps.alloc(3 * map_words));
+	ABB_CUDA(cudaMemsetAsync(f->maps.p, 0, 3 * map_words * sizeof(unsigned), f->stream));
+	for (auto& tags : f->d_tags2) {
+		ABB_CHECK(tags.alloc(f->tag_slots));
+		ABB_CUDA(cudaMemsetAsync(tags.p, 0, f->tag_slots * sizeof(unsigned long long), f->stream));
 	}
 	// worst case everything defers: window slots + the carried lanes, twice, plus the drain's sorted copy
-	ABB_CUDA(cudaMalloc((void**)&f->d_carry, 3 * (f->window + kCarryLanes) * sizeof(uint64_t)));
+	ABB_CHECK(f->d_carry.alloc(3 * (f->window + kCarryLanes)));
 	// presence bitmap of the drain: pending slots span at most age_off + 2 windows
 	f->slotbit_words = ((uint64_t)age_windows_for(f->window) + 3) * f->window / 32 + 64;
-	ABB_CUDA(cudaMalloc((void**)&f->d_slotbits, f->slotbit_words * sizeof(unsigned)));
-	ABB_CUDA(cudaMemsetAsync(f->d_slotbits, 0, f->slotbit_words * sizeof(unsigned), f->stream));
+	ABB_CHECK(f->d_slotbits.alloc(f->slotbit_words));
+	ABB_CUDA(cudaMemsetAsync(f->d_slotbits.p, 0, f->slotbit_words * sizeof(unsigned), f->stream));
+	for (int i = 0; i < 3; ++i)
+		f->d_map[i] = f->maps.p + i * map_words;
+	f->map_entries = want_entries;
 	f->ws_window = f->window;
 	f->ws_H = f->H;
 	return ABB_OK;
@@ -236,7 +235,7 @@ static int ordered_insert(abb_filter* f, const uint64_t* d_hashes, const uint8_t
 		return ABB_OK;
 	if (f->kind == ABB_BIT) {
 		ABB_DISPATCH_H(f->H, (k_bits_insert<LITERAL, MAXH><<<blocks_for(n_slots, 256), 256, 0, f->stream>>>(
-		                         d_hashes, d_valid, n_slots, f->cfg, f->d_data)));
+		                         d_hashes, d_valid, n_slots, f->cfg, f->d_data.p)));
 		f->st.launches += 1;
 		ABB_CUDA(cudaGetLastError());
 		return ABB_OK;
@@ -260,22 +259,22 @@ static int ordered_insert(abb_filter* f, const uint64_t* d_hashes, const uint8_t
 		a.map[i].mask = f->map_entries - 1;
 	}
 	for (int i = 0; i < 2; ++i) {
-		a.tags[i] = f->d_tags2[i];
-		a.carry[i] = f->d_carry + (uint64_t)i * cap;
+		a.tags[i] = f->d_tags2[i].p;
+		a.carry[i] = f->d_carry.p + (uint64_t)i * cap;
 	}
 	a.tag_cap = (unsigned)f->tag_slots;
 	a.f = view_of(f);
 	a.age_off = (unsigned)(age_windows_for(W) * W);
 	a.drain_age = a.age_off / 3 * 2;
-	a.ctl = reinterpret_cast<InsertCtl*>(f->d_ctl);
-	a.stats = f->d_stats;
+	a.ctl = reinterpret_cast<InsertCtl*>(f->d_ctl.p);
+	a.stats = f->d_stats.p;
 	a.dbg = getenv("ABB_DBG") ? (unsigned)atoi(getenv("ABB_DBG")) : 0u;
-	uint64_t* sorted = f->d_carry + 2 * cap;
+	uint64_t* sorted = f->d_carry.p + 2 * cap;
 	// the maps, both tag tables and the control block start clean
-	ABB_CUDA(cudaMemsetAsync(f->d_ctl, 0, sizeof(InsertCtl), st));
+	ABB_CUDA(cudaMemsetAsync(f->d_ctl.p, 0, sizeof(InsertCtl), st));
 	ABB_CUDA(cudaMemsetAsync(f->d_map[0], 0, 3 * std::max<size_t>(f->map_entries / 4, 256), st));
 	for (int i = 0; i < 2; ++i)
-		ABB_CUDA(cudaMemsetAsync(f->d_tags2[i], 0, f->tag_slots * sizeof(unsigned long long), st));
+		ABB_CUDA(cudaMemsetAsync(f->d_tags2[i].p, 0, f->tag_slots * sizeof(unsigned long long), st));
 	const bool counting = f->kind == ABB_COUNTING;
 	PolicyHold policy(f, 3);
 	while (a.w_begin < a.n_windows) {
@@ -291,7 +290,7 @@ static int ordered_insert(abb_filter* f, const uint64_t* d_hashes, const uint8_t
 		if (timed)
 			cudaEventRecord(f->prof_ev[f->prof_used++], st);
 		InsertCtl h;
-		ABB_CUDA(cudaMemcpyAsync(&h, f->d_ctl, sizeof h, cudaMemcpyDeviceToHost, st));
+		ABB_CUDA(cudaMemcpyAsync(&h, f->d_ctl.p, sizeof h, cudaMemcpyDeviceToHost, st));
 		ABB_CUDA(cudaStreamSynchronize(st));
 		ABB_REQUIRE(h.resume > a.w_begin && h.resume <= a.n_windows, "insert kernel made no progress (window %u of %u)", h.resume, a.n_windows);
 		if (timed)
@@ -302,11 +301,11 @@ static int ordered_insert(abb_filter* f, const uint64_t* d_hashes, const uint8_t
 		const uint64_t lo_slot = w0 > (uint64_t)a.age_off + W ? w0 - a.age_off - W : 0;
 		ABB_DISPATCH_H(f->H, {
 			if (counting)
-				k_drain<0, LITERAL, MAXH><<<1, kDrainThreads, 0, st>>>(d_hashes, f->cfg, a.f, a.carry[which], a.ctl, which, 0, 1, f->d_slotbits, lo_slot,
-				                                                      sorted, f->d_stats);
+				k_drain<0, LITERAL, MAXH><<<1, kDrainThreads, 0, st>>>(d_hashes, f->cfg, a.f, a.carry[which], a.ctl, which, 0, 1, f->d_slotbits.p, lo_slot,
+				                                                      sorted, f->d_stats.p);
 			else
-				k_drain<1, LITERAL, MAXH><<<1, kDrainThreads, 0, st>>>(d_hashes, f->cfg, a.f, a.carry[which], a.ctl, which, 0, 1, f->d_slotbits, lo_slot,
-				                                                      sorted, f->d_stats);
+				k_drain<1, LITERAL, MAXH><<<1, kDrainThreads, 0, st>>>(d_hashes, f->cfg, a.f, a.carry[which], a.ctl, which, 0, 1, f->d_slotbits.p, lo_slot,
+				                                                      sorted, f->d_stats.p);
 		});
 		f->st.launches += 2;
 		f->st.windows += h.resume - a.w_begin;
@@ -488,7 +487,7 @@ static int insert_reads_dev(abb_filter* f, const uint8_t* d_bases, const uint64_
 		bounds = { 0, n_reads };
 	} else {
 		const unsigned max_chunks = (unsigned)(total / kChunkSlots + 3) * 2;
-		// a member buffer: a cudaMalloc / cudaFree per call would synchronise the device, i.e. wait for the host-to-device copy
+		// a member buffer: an allocation and free per call would synchronise the device, i.e. wait for the host-to-device copy
 		// that abb_insert_reads runs next to this insert
 		DevBuf<uint64_t>& d_bounds = f->bounds;
 		ABB_CHECK(d_bounds.reserve(max_chunks + 2));
@@ -507,7 +506,7 @@ static int insert_reads_dev(abb_filter* f, const uint8_t* d_bases, const uint64_
 		ABB_CUDA(cudaMemcpyAsync(&slot_at[i], f->slot_offs.p + bounds[i], sizeof(uint64_t), cudaMemcpyDeviceToHost, f->stream));
 	ABB_CUDA(cudaStreamSynchronize(f->stream));
 
-	ABB_CUDA(cudaMemsetAsync(f->d_stats + 3, 0, sizeof(unsigned long long), f->stream));
+	ABB_CUDA(cudaMemsetAsync(f->d_stats.p + 3, 0, sizeof(unsigned long long), f->stream));
 	for (size_t c = 0; c + 1 < bounds.size(); ++c) {
 		const uint64_t r0 = bounds[c], r1 = bounds[c + 1];
 		const uint64_t slots = slot_at[c + 1] - slot_at[c];
@@ -518,9 +517,9 @@ static int insert_reads_dev(abb_filter* f, const uint8_t* d_bases, const uint64_
 		if (pc)
 			ABB_CHECK(wait_bases(f, pc, pc->h_offs[r1]));
 		ABB_CUDA(cudaEventRecord(f->ev0, f->stream));
-		ABB_CHECK(launch_hash(f, f->k, f->d_care, d_bases, d_offs, f->slot_offs.p, r0, r1, slot_at[c], f->h0.p, f->valid.p,
+		ABB_CHECK(launch_hash(f, f->k, f->d_care.p, d_bases, d_offs, f->slot_offs.p, r0, r1, slot_at[c], f->h0.p, f->valid.p,
 		                      f->stream, &f->st.launches));
-		k_count_valid<<<std::min<unsigned>(blocks_for(slots, 256), sm_count() * 8), 256, 0, f->stream>>>(f->valid.p, slots, f->d_stats + 3);
+		k_count_valid<<<std::min<unsigned>(blocks_for(slots, 256), sm_count() * 8), 256, 0, f->stream>>>(f->valid.p, slots, f->d_stats.p + 3);
 		f->st.launches += 1;
 		ABB_CUDA(cudaEventRecord(f->ev1, f->stream));
 		if (comm)
@@ -539,7 +538,7 @@ static int insert_reads_dev(abb_filter* f, const uint8_t* d_bases, const uint64_
 		f->st.slots += slots;
 	}
 	unsigned long long nk = 0;
-	ABB_CUDA(cudaMemcpyAsync(&nk, f->d_stats + 3, sizeof nk, cudaMemcpyDeviceToHost, f->stream));
+	ABB_CUDA(cudaMemcpyAsync(&nk, f->d_stats.p + 3, sizeof nk, cudaMemcpyDeviceToHost, f->stream));
 	ABB_CUDA(cudaStreamSynchronize(f->stream));
 	f->st.kmers += nk;
 	if (n_kmers_out)
@@ -650,9 +649,9 @@ static int sharded_ordered_insert(abb_filter* f, abb_comm* c, const uint64_t* d_
 	const unsigned age_off = (unsigned)(age_windows_for(W) * W);
 	const unsigned drain_age = age_off / 3 * 2;
 	const uint64_t cap = 3 * (W + kCarryLanes) / 2; // two lists in the allocation of three (no drain list is needed here)
-	uint64_t* carry[2] = { f->d_carry, f->d_carry + cap };
-	ShardCtl* ctl = reinterpret_cast<ShardCtl*>(f->d_ctl);
-	unsigned* d_nout = f->d_ctl + 4; // [n_out]; the ctl block has 8 words
+	uint64_t* carry[2] = { f->d_carry.p, f->d_carry.p + cap };
+	ShardCtl* ctl = reinterpret_cast<ShardCtl*>(f->d_ctl.p);
+	unsigned* d_nout = f->d_ctl.p + 4; // [n_out]; the ctl block has 8 words
 	const size_t map_bytes = std::max<size_t>(f->map_entries / 4, 256);
 	ConflictMap maps[2] = { { f->d_map[0], f->map_entries - 1 }, { f->d_map[1], f->map_entries - 1 } };
 	const uint64_t chunk = shard_chunk(f->size, (unsigned)c->world);
@@ -679,7 +678,7 @@ static int sharded_ordered_insert(abb_filter* f, abb_comm* c, const uint64_t* d_
 		uint64_t tslots = 4096;
 		while (tslots < 8ULL * lanes_c * f->H / (unsigned)c->world + 4096 && tslots < f->tag_slots)
 			tslots <<= 1;
-		const TagTable tab = { f->d_tags2[0], std::min<uint64_t>(tslots, f->tag_slots) - 1 };
+		const TagTable tab = { f->d_tags2[0].p, std::min<uint64_t>(tslots, f->tag_slots) - 1 };
 		if (lanes_c)
 			ABB_CUDA(cudaMemsetAsync(tab.e, 0, (tab.mask + 1) * sizeof(unsigned long long), st));
 		const unsigned lanes = lanes_c + n;
@@ -693,18 +692,18 @@ static int sharded_ordered_insert(abb_filter* f, abb_comm* c, const uint64_t* d_
 			if (timed)
 				cudaEventRecord(f->prof_ev[f->prof_used++], st);
 			k_sh_gather<false, MAXH><<<blocks_for((uint64_t)lanes_c + std::max(n, n_next), 256), 256, 0, st>>>(
-			    d_h0, d_valid, w0, n, w1, n_next, f->cfg, maps[p], maps[1 - p], tab, f->d_data, age_off, carry[in], lanes_c, sh, pm, ok);
+			    d_h0, d_valid, w0, n, w1, n_next, f->cfg, maps[p], maps[1 - p], tab, f->d_data.p, age_off, carry[in], lanes_c, sh, pm, ok);
 		});
 		if (lanes) {
 			ABB_NCCL(g_nccl.AllReduce(buf, buf, 2 * (size_t)lanes, ncclUint8, ncclMin, c->comm, st));
 			ABB_DISPATCH_H(f->H, (k_sh_apply<false, MAXH><<<blocks_for((uint64_t)n_in + n, 256), 256, 0, st>>>(
-			                         d_h0, d_valid, w0, n, f->cfg, tab, f->d_data, carry[in], n_in, lanes_c, sh, pm, ok, f->d_slotbits, lo_slot, ctl,
-			                         f->d_stats)));
+			                         d_h0, d_valid, w0, n, f->cfg, tab, f->d_data.p, carry[in], n_in, lanes_c, sh, pm, ok, f->d_slotbits.p, lo_slot, ctl,
+			                         f->d_stats.p)));
 			if (timed) {
 				cudaEventRecord(f->prof_ev[f->prof_used++], st);
 				f->prof_slots += n;
 			}
-			k_sh_compact<<<1, kDrainThreads, 0, st>>>(f->d_slotbits, lo_slot, w0 + std::max<uint64_t>(n, 1), carry[1 - in], ctl, d_nout);
+			k_sh_compact<<<1, kDrainThreads, 0, st>>>(f->d_slotbits.p, lo_slot, w0 + std::max<uint64_t>(n, 1), carry[1 - in], ctl, d_nout);
 			unsigned h_n = 0;
 			ABB_CUDA(cudaMemcpyAsync(&h_n, d_nout, sizeof h_n, cudaMemcpyDeviceToHost, st));
 			if (h_n || true) // the oldest pending slot bounds the priorities
@@ -761,7 +760,7 @@ static int sharded_ordered_insert(abb_filter* f, abb_comm* c, const uint64_t* d_
 		f->prof_slots = 0;
 	}
 	// leave the shared control block in the single-GPU layout
-	ABB_CUDA(cudaMemsetAsync(f->d_ctl, 0, 8 * sizeof(unsigned), st));
+	ABB_CUDA(cudaMemsetAsync(f->d_ctl.p, 0, 8 * sizeof(unsigned), st));
 	return ABB_OK;
 }
 
@@ -788,7 +787,7 @@ int abb_device_count(void)
 	return n;
 }
 
-static int alloc_filter(abb_filter* f, abb_filter** out);
+static int alloc_filter(std::unique_ptr<abb_filter> f, abb_filter** out);
 
 int abb_filter_create(abb_filter** out, int kind, uint64_t size, unsigned num_hashes, unsigned k, unsigned arg,
                       const char* mask, int device)
@@ -825,7 +824,7 @@ int abb_filter_create(abb_filter** out, int kind, uint64_t size, unsigned num_ha
 	}
 	ABB_CHECK(select_device(device));
 
-	abb_filter* f = new (std::nothrow) abb_filter();
+	std::unique_ptr<abb_filter> f(new (std::nothrow) abb_filter());
 	if (!f) {
 		set_error("out of host memory");
 		return ABB_ENOMEM;
@@ -845,46 +844,32 @@ int abb_filter_create(abb_filter** out, int kind, uint64_t size, unsigned num_ha
 	f->cfg.mod = make_fastmod(size);
 	for (unsigned i = 0; i < kMaxHashes; ++i)
 		f->cfg.mult[i] = (uint64_t)i ^ ((uint64_t)k * kMultiSeed); // nthash.hpp:339
-	return alloc_filter(f, out);
+	return alloc_filter(std::move(f), out);
 }
 
-/** the device side of a filter whose geometry is set: stream, events, the zeroed levels, control words.  Frees f on failure. */
-static int alloc_filter(abb_filter* f, abb_filter** out)
+/** the device side of a filter whose geometry is set: stream, events, the zeroed levels, control words */
+static int alloc_filter(std::unique_ptr<abb_filter> f, abb_filter** out)
 {
 	const unsigned k = f->k, levels = f->levels;
-	auto fail = [&](int rc) {
-		abb_filter_destroy(f);
-		return rc;
-	};
-#define ABB_TRY(call)                                                                 \
-	do {                                                                              \
-		cudaError_t e__ = (call);                                                     \
-		if (e__ != cudaSuccess) {                                                     \
-			set_error("%s failed: %s", #call, cudaGetErrorString(e__));               \
-			return fail(e__ == cudaErrorMemoryAllocation ? ABB_ENOMEM : ABB_ECUDA);   \
-		}                                                                             \
-	} while (0)
-	ABB_TRY(cudaStreamCreateWithFlags(&f->stream, cudaStreamNonBlocking));
-	ABB_TRY(cudaEventCreate(&f->ev0));
-	ABB_TRY(cudaEventCreate(&f->ev1));
+	ABB_CUDA(cudaStreamCreateWithFlags(f->stream.out(), cudaStreamNonBlocking));
+	ABB_CUDA(cudaEventCreate(f->ev0.out()));
+	ABB_CUDA(cudaEventCreate(f->ev1.out()));
 	// slack: the in-place all-gather of position shards rounds each shard up to 16 bytes (abb_filter_allgather)
-	ABB_TRY(cudaMalloc((void**)&f->d_data, f->bytes_per_level * levels + 4096));
-	ABB_TRY(cudaMemsetAsync(f->d_data, 0, f->bytes_per_level * levels, f->stream));
-	ABB_TRY(cudaMalloc((void**)&f->d_ctl, 8 * sizeof(unsigned)));
-	ABB_TRY(cudaMemsetAsync(f->d_ctl, 0, 8 * sizeof(unsigned), f->stream));
-	ABB_TRY(cudaMalloc((void**)&f->d_stats, 8 * sizeof(unsigned long long)));
-	ABB_TRY(cudaMemsetAsync(f->d_stats, 0, 8 * sizeof(unsigned long long), f->stream));
+	ABB_CHECK(f->d_data.alloc(f->bytes_per_level * levels + 4096));
+	ABB_CUDA(cudaMemsetAsync(f->d_data.p, 0, f->bytes_per_level * levels, f->stream));
+	ABB_CHECK(f->d_ctl.alloc(8));
+	ABB_CUDA(cudaMemsetAsync(f->d_ctl.p, 0, 8 * sizeof(unsigned), f->stream));
+	ABB_CHECK(f->d_stats.alloc(8));
+	ABB_CUDA(cudaMemsetAsync(f->d_stats.p, 0, 8 * sizeof(unsigned long long), f->stream));
 	if (!f->mask.empty()) {
 		std::vector<uint8_t> care(k);
 		for (unsigned i = 0; i < k; ++i)
 			care[i] = f->mask[i] == '1';
-		ABB_TRY(cudaMalloc((void**)&f->d_care, k));
-		ABB_TRY(cudaMemcpyAsync(f->d_care, care.data(), k, cudaMemcpyHostToDevice, f->stream));
+		ABB_CHECK(f->d_care.alloc(k));
+		ABB_CUDA(cudaMemcpyAsync(f->d_care.p, care.data(), k, cudaMemcpyHostToDevice, f->stream));
 	}
-	ABB_TRY(cudaStreamSynchronize(f->stream));
-#undef ABB_TRY
-	*out = f;
-	return ABB_OK;
+	ABB_CUDA(cudaStreamSynchronize(f->stream));
+	return hand_over(f, out);
 }
 
 int abb_konnector_create(abb_filter** out, uint64_t full_bits, unsigned k, unsigned levels, uint64_t hash_seed, uint64_t start_bit,
@@ -898,7 +883,7 @@ int abb_konnector_create(abb_filter** out, uint64_t full_bits, unsigned k, unsig
 	            (unsigned long long)start_bit, (unsigned long long)end_bit, (unsigned long long)full_bits);
 	ABB_REQUIRE(levels >= 1 && levels <= 255, "a Konnector filter needs 1..255 levels");
 	ABB_CHECK(select_device(device));
-	abb_filter* f = new (std::nothrow) abb_filter();
+	std::unique_ptr<abb_filter> f(new (std::nothrow) abb_filter());
 	if (!f) {
 		set_error("out of host memory");
 		return ABB_ENOMEM;
@@ -913,7 +898,7 @@ int abb_konnector_create(abb_filter** out, uint64_t full_bits, unsigned k, unsig
 	f->kon_full = full_bits;
 	f->kon_start = start_bit;
 	f->kon_seed = hash_seed;
-	return alloc_filter(f, out);
+	return alloc_filter(std::move(f), out);
 }
 
 int abb_filter_destroy(abb_filter* f)
@@ -921,45 +906,9 @@ int abb_filter_destroy(abb_filter* f)
 	if (!f)
 		return ABB_OK;
 	cudaSetDevice(f->device);
-	if (f->stream)
-		cudaStreamSynchronize(f->stream);
-	cudaFree(f->d_data);
-	cudaFree(f->d_care);
-	cudaFree(f->d_tags2[0]);
-	cudaFree(f->d_tags2[1]);
-	cudaFree(f->d_map[0]); // holds both maps
-	cudaFree(f->d_carry);
-	cudaFree(f->d_slotbits);
-	cudaFree(f->d_ctl);
-	cudaFree(f->d_stats);
-	f->bases.release();
-	f->offs.release();
-	f->slot_offs.release();
-	f->h0.release();
-	f->lit.release();
-	f->bounds.release();
-	f->gq_kmers.release();
-	f->gq_info.release();
-	f->gq_len.release();
-	f->gq_self.release();
-	f->valid.release();
-	f->scan_tmp.release();
-	f->out8.release();
-	f->sh_buf.release();
-	for (auto e : f->prof_ev)
-		cudaEventDestroy(e);
-	if (f->ev0)
-		cudaEventDestroy(f->ev0);
-	if (f->ev1)
-		cudaEventDestroy(f->ev1);
-	for (auto e : f->copy_ev)
-		cudaEventDestroy(e);
-	if (f->copy_stream) {
+	cudaStreamSynchronize(f->stream);
+	if (f->copy_stream)
 		cudaStreamSynchronize(f->copy_stream);
-		cudaStreamDestroy(f->copy_stream);
-	}
-	if (f->stream)
-		cudaStreamDestroy(f->stream);
 	delete f;
 	return ABB_OK;
 }
@@ -988,9 +937,10 @@ int abb_filter_set_profiling(abb_filter* f, int on)
 	ABB_CUDA(cudaSetDevice(f->device));
 	f->profile = on != 0;
 	if (f->profile && f->prof_ev.empty()) {
-		f->prof_ev.resize(2048);
-		for (auto& e : f->prof_ev)
-			ABB_CUDA(cudaEventCreate(&e));
+		std::vector<Event> ev(2048); // kept only if every create succeeds: an empty prof_ev is retried on the next call
+		for (auto& e : ev)
+			ABB_CUDA(cudaEventCreate(e.out()));
+		f->prof_ev = std::move(ev);
 	}
 	return ABB_OK;
 }
@@ -1052,7 +1002,7 @@ int abb_insert_reads(abb_filter* f, const char* bases, const uint64_t* offsets, 
 		return insert_reads_dev(f, f->bases.p, f->offs.p, n_reads, n_kmers_out);
 	}
 	if (!f->copy_stream)
-		ABB_CUDA(cudaStreamCreateWithFlags(&f->copy_stream, cudaStreamNonBlocking));
+		ABB_CUDA(cudaStreamCreateWithFlags(f->copy_stream.out(), cudaStreamNonBlocking));
 	if (f->kind != ABB_BIT)
 		ABB_CHECK(ensure_workspace(f)); // the maps exist before the policy that pins them is set
 	PolicyHold policy(f, 3); // before the copy starts: setting it later would wait for the whole copy (see PolicyHold)
@@ -1061,9 +1011,9 @@ int abb_insert_reads(abb_filter* f, const char* bases, const uint64_t* offsets, 
 	pc.piece = kPiece;
 	pc.n_pieces = (size_t)((n_bases + kPiece - 1) / kPiece);
 	while (f->copy_ev.size() < pc.n_pieces) {
-		cudaEvent_t ev;
-		ABB_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-		f->copy_ev.push_back(ev);
+		Event ev;
+		ABB_CUDA(cudaEventCreateWithFlags(ev.out(), cudaEventDisableTiming));
+		f->copy_ev.push_back(std::move(ev));
 	}
 	// the destination may still be read by work queued on the filter's stream (pass 2 of a previous job)
 	ABB_CUDA(cudaEventRecord(f->ev0, f->stream));
@@ -1177,7 +1127,7 @@ int abb_hash_reads_dev(abb_filter* f, const char* d_bases, const uint64_t* d_off
 	if (total == 0 || !d_h0 || !d_valid)
 		return ABB_OK;
 	ABB_REQUIRE(capacity >= total, "output buffers hold %llu slots, %llu needed", (unsigned long long)capacity, (unsigned long long)total);
-	ABB_CHECK(launch_hash(f, f->k, f->d_care, (const uint8_t*)d_bases, d_offsets, f->slot_offs.p, 0, n_reads, 0, d_h0, d_valid, f->stream,
+	ABB_CHECK(launch_hash(f, f->k, f->d_care.p, (const uint8_t*)d_bases, d_offsets, f->slot_offs.p, 0, n_reads, 0, d_h0, d_valid, f->stream,
 	                      &f->st.launches));
 	ABB_CUDA(cudaStreamSynchronize(f->stream));
 	return ABB_OK;
@@ -1245,7 +1195,7 @@ int abb_filter_allgather(abb_filter* f, abb_comm* c)
 		return ABB_OK;
 	const uint64_t chunk = shard_chunk(f->bytes_per_level, (unsigned)c->world);
 	ABB_REQUIRE(chunk * c->world <= f->bytes_per_level + 4096, "too many ranks for the all-gather slack");
-	ABB_NCCL(g_nccl.AllGather(f->d_data + (uint64_t)c->rank * chunk, f->d_data, chunk, ncclUint8, c->comm, f->stream));
+	ABB_NCCL(g_nccl.AllGather(f->d_data.p + (uint64_t)c->rank * chunk, f->d_data.p, chunk, ncclUint8, c->comm, f->stream));
 	ABB_CUDA(cudaStreamSynchronize(f->stream));
 	return ABB_OK;
 }
@@ -1323,7 +1273,7 @@ void* abb_filter_device_ptr(abb_filter* f, int level)
 		return nullptr;
 	cudaSetDevice(f->device);
 	cudaStreamSynchronize(f->stream);
-	return f->d_data + (uint64_t)level * f->bytes_per_level;
+	return f->d_data.p + (uint64_t)level * f->bytes_per_level;
 }
 
 static int query_hashes(abb_filter* f, const uint64_t* hashes, uint64_t n, uint8_t* out, bool want_min)
@@ -1369,52 +1319,40 @@ int abb_contains_reads(abb_filter* f, const char* bases, const uint64_t* offsets
 	// own staging buffers: the batch a previous insert left resident (abb_filter_resident_reads) stays valid
 	DevBuf<uint8_t> d_bases;
 	DevBuf<uint64_t> d_offs;
-	auto done = [&](int rc) {
-		d_bases.release();
-		d_offs.release();
-		return rc;
-	};
-	int rc = d_bases.reserve(n_bases + 16);
-	if (rc == ABB_OK)
-		rc = d_offs.reserve(n_reads + 1);
-	if (rc != ABB_OK)
-		return done(rc);
-	auto run = [&]() -> int {
-		ABB_CUDA(cudaMemcpyAsync(d_bases.p, bases, n_bases, cudaMemcpyHostToDevice, f->stream));
-		ABB_CUDA(cudaMemcpyAsync(d_offs.p, offsets, (n_reads + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, f->stream));
-		uint64_t total = 0;
-		ABB_CHECK(compute_slot_offsets(f->k, d_offs.p, n_reads, f->slot_offs, f->scan_tmp, f->stream, &total, &f->st.launches));
-		if (n_slots_out)
-			*n_slots_out = total;
-		if (total == 0 || (!out_flag && !out_valid))
-			return ABB_OK;
-		ABB_REQUIRE(capacity >= total, "output buffers hold %llu slots, %llu needed", (unsigned long long)capacity, (unsigned long long)total);
-		ABB_CHECK(f->valid.reserve(total));
-		ABB_CHECK(f->out8.reserve(total));
-		if (f->kind == ABB_KONNECTOR)
-			ABB_CHECK(kon_query_slots(f, d_bases.p, d_offs.p, n_reads, total));
-		else {
-			ABB_CHECK(f->h0.reserve(total));
-			ABB_CHECK(launch_hash(f, f->k, f->d_care, d_bases.p, d_offs.p, f->slot_offs.p, 0, n_reads, 0, f->h0.p, f->valid.p, f->stream, &f->st.launches));
-			const FilterView fv = view_of(f);
-			const unsigned grid = std::min<unsigned>(blocks_for(total, 256), sm_count() * 16);
-			if (f->kind == ABB_COUNTING)
-				k_query_h0<0><<<grid, 256, 0, f->stream>>>(f->h0.p, f->valid.p, total, f->cfg, fv, f->threshold, f->out8.p);
-			else
-				k_query_h0<1><<<grid, 256, 0, f->stream>>>(f->h0.p, f->valid.p, total, f->cfg, fv, 0, f->out8.p);
-			f->st.launches += 1;
-			ABB_CUDA(cudaGetLastError());
-		}
-		if (out_flag)
-			ABB_CUDA(cudaMemcpyAsync(out_flag, f->out8.p, total, cudaMemcpyDeviceToHost, f->stream));
-		if (out_valid)
-			ABB_CUDA(cudaMemcpyAsync(out_valid, f->valid.p, total, cudaMemcpyDeviceToHost, f->stream));
-		ABB_CUDA(cudaStreamSynchronize(f->stream));
+	ABB_CHECK(d_bases.reserve(n_bases + 16));
+	ABB_CHECK(d_offs.reserve(n_reads + 1));
+	const SyncOnExit sync = { f->stream }; // before the staging buffers are freed
+	ABB_CUDA(cudaMemcpyAsync(d_bases.p, bases, n_bases, cudaMemcpyHostToDevice, f->stream));
+	ABB_CUDA(cudaMemcpyAsync(d_offs.p, offsets, (n_reads + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, f->stream));
+	uint64_t total = 0;
+	ABB_CHECK(compute_slot_offsets(f->k, d_offs.p, n_reads, f->slot_offs, f->scan_tmp, f->stream, &total, &f->st.launches));
+	if (n_slots_out)
+		*n_slots_out = total;
+	if (total == 0 || (!out_flag && !out_valid))
 		return ABB_OK;
-	};
-	rc = run();
-	cudaStreamSynchronize(f->stream);
-	return done(rc);
+	ABB_REQUIRE(capacity >= total, "output buffers hold %llu slots, %llu needed", (unsigned long long)capacity, (unsigned long long)total);
+	ABB_CHECK(f->valid.reserve(total));
+	ABB_CHECK(f->out8.reserve(total));
+	if (f->kind == ABB_KONNECTOR)
+		ABB_CHECK(kon_query_slots(f, d_bases.p, d_offs.p, n_reads, total));
+	else {
+		ABB_CHECK(f->h0.reserve(total));
+		ABB_CHECK(launch_hash(f, f->k, f->d_care.p, d_bases.p, d_offs.p, f->slot_offs.p, 0, n_reads, 0, f->h0.p, f->valid.p, f->stream, &f->st.launches));
+		const FilterView fv = view_of(f);
+		const unsigned grid = std::min<unsigned>(blocks_for(total, 256), sm_count() * 16);
+		if (f->kind == ABB_COUNTING)
+			k_query_h0<0><<<grid, 256, 0, f->stream>>>(f->h0.p, f->valid.p, total, f->cfg, fv, f->threshold, f->out8.p);
+		else
+			k_query_h0<1><<<grid, 256, 0, f->stream>>>(f->h0.p, f->valid.p, total, f->cfg, fv, 0, f->out8.p);
+		f->st.launches += 1;
+		ABB_CUDA(cudaGetLastError());
+	}
+	if (out_flag)
+		ABB_CUDA(cudaMemcpyAsync(out_flag, f->out8.p, total, cudaMemcpyDeviceToHost, f->stream));
+	if (out_valid)
+		ABB_CUDA(cudaMemcpyAsync(out_valid, f->valid.p, total, cudaMemcpyDeviceToHost, f->stream));
+	ABB_CUDA(cudaStreamSynchronize(f->stream));
+	return ABB_OK;
 }
 
 int abb_successors(abb_filter* f, const char* kmers, uint64_t n, unsigned max_chain, abb_succ_info* out, unsigned* out_len, uint64_t* self_hash)
@@ -1432,32 +1370,28 @@ int abb_successors(abb_filter* f, const char* kmers, uint64_t n, unsigned max_ch
 	DevBuf<abb_succ_info>& d_info = f->gq_info;
 	DevBuf<unsigned>& d_len = f->gq_len;
 	DevBuf<uint64_t>& d_self = f->gq_self;
-	auto run = [&]() -> int {
-		ABB_CHECK(d_k.reserve(n * f->k));
-		ABB_CHECK(d_info.reserve(n * max_chain));
-		ABB_CHECK(d_len.reserve(n));
-		ABB_CHECK(d_self.reserve(n));
-		ABB_CUDA(cudaMemcpyAsync(d_k.p, kmers, n * f->k, cudaMemcpyHostToDevice, f->stream));
-		ABB_CUDA(cudaMemsetAsync(d_info.p, 0, n * max_chain * sizeof(abb_succ_info), f->stream));
-		const FilterView fv = view_of(f);
-		if (f->kind == ABB_COUNTING) {
-			const FilterProbe<0> probe = { f->cfg, fv, f->threshold };
-			k_successors<0><<<blocks_for(n, 128), 128, 0, f->stream>>>(d_k.p, n, f->k, max_chain, probe, d_info.p, d_len.p, d_self.p);
-		} else {
-			const FilterProbe<1> probe = { f->cfg, fv, 0 };
-			k_successors<1><<<blocks_for(n, 128), 128, 0, f->stream>>>(d_k.p, n, f->k, max_chain, probe, d_info.p, d_len.p, d_self.p);
-		}
-		f->st.launches += 1;
-		ABB_CUDA(cudaGetLastError());
-		ABB_CUDA(cudaMemcpyAsync(out, d_info.p, n * max_chain * sizeof(abb_succ_info), cudaMemcpyDeviceToHost, f->stream));
-		ABB_CUDA(cudaMemcpyAsync(out_len, d_len.p, n * sizeof(unsigned), cudaMemcpyDeviceToHost, f->stream));
-		ABB_CUDA(cudaMemcpyAsync(self_hash, d_self.p, n * sizeof(uint64_t), cudaMemcpyDeviceToHost, f->stream));
-		ABB_CUDA(cudaStreamSynchronize(f->stream));
-		return ABB_OK;
-	};
-	const int rc = run();
-	cudaStreamSynchronize(f->stream);
-	return rc;
+	const SyncOnExit sync = { f->stream };
+	ABB_CHECK(d_k.reserve(n * f->k));
+	ABB_CHECK(d_info.reserve(n * max_chain));
+	ABB_CHECK(d_len.reserve(n));
+	ABB_CHECK(d_self.reserve(n));
+	ABB_CUDA(cudaMemcpyAsync(d_k.p, kmers, n * f->k, cudaMemcpyHostToDevice, f->stream));
+	ABB_CUDA(cudaMemsetAsync(d_info.p, 0, n * max_chain * sizeof(abb_succ_info), f->stream));
+	const FilterView fv = view_of(f);
+	if (f->kind == ABB_COUNTING) {
+		const FilterProbe<0> probe = { f->cfg, fv, f->threshold };
+		k_successors<0><<<blocks_for(n, 128), 128, 0, f->stream>>>(d_k.p, n, f->k, max_chain, probe, d_info.p, d_len.p, d_self.p);
+	} else {
+		const FilterProbe<1> probe = { f->cfg, fv, 0 };
+		k_successors<1><<<blocks_for(n, 128), 128, 0, f->stream>>>(d_k.p, n, f->k, max_chain, probe, d_info.p, d_len.p, d_self.p);
+	}
+	f->st.launches += 1;
+	ABB_CUDA(cudaGetLastError());
+	ABB_CUDA(cudaMemcpyAsync(out, d_info.p, n * max_chain * sizeof(abb_succ_info), cudaMemcpyDeviceToHost, f->stream));
+	ABB_CUDA(cudaMemcpyAsync(out_len, d_len.p, n * sizeof(unsigned), cudaMemcpyDeviceToHost, f->stream));
+	ABB_CUDA(cudaMemcpyAsync(self_hash, d_self.p, n * sizeof(uint64_t), cudaMemcpyDeviceToHost, f->stream));
+	ABB_CUDA(cudaStreamSynchronize(f->stream));
+	return ABB_OK;
 }
 
 int abb_hash_reads(unsigned k, const char* mask, const char* bases, const uint64_t* offsets, uint64_t n_reads,
@@ -1479,41 +1413,29 @@ int abb_hash_reads(unsigned k, const char* mask, const char* bases, const uint64
 	const uint64_t n_bases = offsets[n_reads];
 	DevBuf<uint8_t> d_bases, d_valid, tmp, d_care;
 	DevBuf<uint64_t> d_offs, d_slot, d_h0;
-	int rc = ABB_OK;
-	auto cleanup = [&]() {
-		d_bases.release(); d_valid.release(); tmp.release(); d_care.release();
-		d_offs.release(); d_slot.release(); d_h0.release();
-	};
-#define ABB_TRYRC(expr) do { rc = (expr); if (rc != ABB_OK) { cleanup(); return rc; } } while (0)
-	auto cu = [&](cudaError_t e, const char* what) {
-		if (e != cudaSuccess) { set_error("%s: %s", what, cudaGetErrorString(e)); return (int)ABB_ECUDA; }
-		return (int)ABB_OK;
-	};
-	ABB_TRYRC(d_bases.reserve(n_bases + 16));
-	ABB_TRYRC(d_offs.reserve(n_reads + 1));
-	ABB_TRYRC(cu(cudaMemcpy(d_bases.p, bases, n_bases, cudaMemcpyHostToDevice), "H2D bases"));
-	ABB_TRYRC(cu(cudaMemcpy(d_offs.p, offsets, (n_reads + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice), "H2D offsets"));
+	ABB_CHECK(d_bases.reserve(n_bases + 16));
+	ABB_CHECK(d_offs.reserve(n_reads + 1));
+	ABB_CUDA(cudaMemcpy(d_bases.p, bases, n_bases, cudaMemcpyHostToDevice));
+	ABB_CUDA(cudaMemcpy(d_offs.p, offsets, (n_reads + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice));
 	if (!m.empty()) {
 		std::vector<uint8_t> care(k);
 		for (unsigned i = 0; i < k; ++i)
 			care[i] = m[i] == '1';
-		ABB_TRYRC(d_care.reserve(k));
-		ABB_TRYRC(cu(cudaMemcpy(d_care.p, care.data(), k, cudaMemcpyHostToDevice), "H2D mask"));
+		ABB_CHECK(d_care.reserve(k));
+		ABB_CUDA(cudaMemcpy(d_care.p, care.data(), k, cudaMemcpyHostToDevice));
 	}
 	uint64_t total = 0;
-	ABB_TRYRC(compute_slot_offsets(k, d_offs.p, n_reads, d_slot, tmp, 0, &total, nullptr));
+	ABB_CHECK(compute_slot_offsets(k, d_offs.p, n_reads, d_slot, tmp, 0, &total, nullptr));
 	if (n_slots_out)
 		*n_slots_out = total;
 	if (total && out_h0 && out_valid) {
-		ABB_TRYRC(d_h0.reserve(total));
-		ABB_TRYRC(d_valid.reserve(total));
-		ABB_TRYRC(launch_hash(nullptr, k, m.empty() ? nullptr : d_care.p, d_bases.p, d_offs.p, d_slot.p, 0, n_reads, 0, d_h0.p,
+		ABB_CHECK(d_h0.reserve(total));
+		ABB_CHECK(d_valid.reserve(total));
+		ABB_CHECK(launch_hash(nullptr, k, m.empty() ? nullptr : d_care.p, d_bases.p, d_offs.p, d_slot.p, 0, n_reads, 0, d_h0.p,
 		                      d_valid.p, 0, nullptr));
-		ABB_TRYRC(cu(cudaMemcpy(out_h0, d_h0.p, total * sizeof(uint64_t), cudaMemcpyDeviceToHost), "D2H h0"));
-		ABB_TRYRC(cu(cudaMemcpy(out_valid, d_valid.p, total, cudaMemcpyDeviceToHost), "D2H valid"));
+		ABB_CUDA(cudaMemcpy(out_h0, d_h0.p, total * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+		ABB_CUDA(cudaMemcpy(out_valid, d_valid.p, total, cudaMemcpyDeviceToHost));
 	}
-#undef ABB_TRYRC
-	cleanup();
 	return ABB_OK;
 }
 
@@ -1525,7 +1447,7 @@ static int level_ptr(abb_filter* f, int level, uint64_t nbytes, uint8_t** p)
 	ABB_REQUIRE((unsigned)level < f->levels, "level %d out of range", level);
 	ABB_REQUIRE(nbytes == f->bytes_per_level, "buffer is %llu bytes, the filter level is %llu", (unsigned long long)nbytes,
 	            (unsigned long long)f->bytes_per_level);
-	*p = f->d_data + (uint64_t)level * f->bytes_per_level;
+	*p = f->d_data.p + (uint64_t)level * f->bytes_per_level;
 	return ABB_OK;
 }
 
@@ -1555,7 +1477,7 @@ int abb_filter_clear(abb_filter* f)
 {
 	ABB_REQUIRE(f, "NULL filter");
 	ABB_CUDA(cudaSetDevice(f->device));
-	ABB_CUDA(cudaMemsetAsync(f->d_data, 0, f->bytes_per_level * f->levels, f->stream));
+	ABB_CUDA(cudaMemsetAsync(f->d_data.p, 0, f->bytes_per_level * f->levels, f->stream));
 	ABB_CUDA(cudaStreamSynchronize(f->stream));
 	return ABB_OK;
 }
@@ -1573,14 +1495,14 @@ int abb_filter_popcount(abb_filter* f, uint64_t* nonzero, uint64_t* at_or_above_
 		return ABB_OK;
 	}
 	ABB_CUDA(cudaSetDevice(f->device));
-	ABB_CUDA(cudaMemsetAsync(f->d_stats + 4, 0, 2 * sizeof(unsigned long long), f->stream));
+	ABB_CUDA(cudaMemsetAsync(f->d_stats.p + 4, 0, 2 * sizeof(unsigned long long), f->stream));
 	// bit / cascading: population of the LAST level (the one contains() consults)
-	const uint8_t* p = f->d_data + (uint64_t)(f->levels - 1) * f->bytes_per_level;
-	k_popcount<<<sm_count() * 8, 256, 0, f->stream>>>(p, f->bytes_per_level, f->kind == ABB_COUNTING, f->threshold, f->d_stats + 4);
+	const uint8_t* p = f->d_data.p + (uint64_t)(f->levels - 1) * f->bytes_per_level;
+	k_popcount<<<sm_count() * 8, 256, 0, f->stream>>>(p, f->bytes_per_level, f->kind == ABB_COUNTING, f->threshold, f->d_stats.p + 4);
 	f->st.launches += 1;
 	ABB_CUDA(cudaGetLastError());
 	unsigned long long h[2] = { 0, 0 };
-	ABB_CUDA(cudaMemcpyAsync(h, f->d_stats + 4, sizeof h, cudaMemcpyDeviceToHost, f->stream));
+	ABB_CUDA(cudaMemcpyAsync(h, f->d_stats.p + 4, sizeof h, cudaMemcpyDeviceToHost, f->stream));
 	ABB_CUDA(cudaStreamSynchronize(f->stream));
 	if (nonzero)
 		*nonzero = h[0];
@@ -1596,7 +1518,7 @@ int abb_filter_insert_stats(abb_filter* f, abb_insert_stats* out, int reset)
 	ABB_REQUIRE(f, "NULL filter");
 	ABB_CUDA(cudaSetDevice(f->device));
 	unsigned long long h[3] = { 0, 0, 0 };
-	ABB_CUDA(cudaMemcpyAsync(h, f->d_stats, sizeof h, cudaMemcpyDeviceToHost, f->stream));
+	ABB_CUDA(cudaMemcpyAsync(h, f->d_stats.p, sizeof h, cudaMemcpyDeviceToHost, f->stream));
 	ABB_CUDA(cudaStreamSynchronize(f->stream));
 	f->st.deferred = h[0];
 	f->st.drains = h[1] + f->sh_drains;
@@ -1606,7 +1528,7 @@ int abb_filter_insert_stats(abb_filter* f, abb_insert_stats* out, int reset)
 	if (reset) {
 		f->sh_drains = 0;
 		f->st = abb_insert_stats{};
-		ABB_CUDA(cudaMemsetAsync(f->d_stats, 0, 3 * sizeof(unsigned long long), f->stream));
+		ABB_CUDA(cudaMemsetAsync(f->d_stats.p, 0, 3 * sizeof(unsigned long long), f->stream));
 	}
 	return ABB_OK;
 }

@@ -1187,20 +1187,20 @@ using namespace abb;
 // host side
 // =============================================================================================
 struct abb_assembler {
-	abb_filter* solid = nullptr;
-	abb_filter* assembled = nullptr;
+	abb_filter* solid = nullptr; // not owned
+	std::unique_ptr<abb_filter, decltype(&abb_filter_destroy)> assembled{ nullptr, abb_filter_destroy };
 	abb_assembly_params params = {};
 	abb_assembly_counters counters = {};
-	cudaStream_t stream = nullptr;
+	cudaStream_t stream = nullptr; // not owned: solid's stream
 	uint64_t reads_seen = 0;
 	int kw = 0;
 	RollTab rt; // per-k roll constants + spaced-seed positions
-	uint8_t* d_mpos = nullptr;
-	const uint8_t* ext_codes = nullptr; // classification supplied by the caller for the next batch (device)
+	DevBuf<uint8_t> d_mpos;
+	const uint8_t* ext_codes = nullptr; // not owned: classification supplied by the caller for the next batch (device)
 	uint64_t ext_n = 0;
-	abb_comm* comm = nullptr;           // multi-GPU: classification, candidate scans and tile production are sharded over it
+	abb_comm* comm = nullptr;           // not owned; multi-GPU: classification, candidate scans and tile production are sharded over it
 	DevBuf<uint8_t> gather;             // all-gather staging (world x padded slice)
-	const uint8_t* cur_bases = nullptr; // device reads of the batch being processed
+	const uint8_t* cur_bases = nullptr; // not owned: device reads of the batch being processed
 	const uint64_t* cur_offs = nullptr;
 
 	// batch state (device)
@@ -1212,27 +1212,27 @@ struct abb_assembler {
 	DevBuf<Frame> frames;
 	DevBuf<uint64_t> look;
 	unsigned scratch_warps = 0;
-	uint8_t* d_arena = nullptr;
+	DevBuf<uint8_t> d_arena;
 	unsigned long long arena_size = 0;
-	unsigned long long* d_arena_top = nullptr;
-	unsigned* d_nrecs = nullptr;
+	DevBuf<unsigned long long> d_arena_top;
+	DevBuf<unsigned> d_nrecs;
 	// contigEndKmers
-	unsigned long long* d_ends = nullptr;
+	DevBuf<unsigned long long> d_ends;
 	unsigned ends_cap = 0;
-	unsigned* d_ends_n = nullptr;
+	DevBuf<unsigned> d_ends_n;
 	uint64_t ends_upper = 0; // upper bound on entries
 
 	// tile store (abb_walk.cuh "Tiles"); persistent across batches
 	bool tiles_on = true;
-	TileRec* d_tiles = nullptr;
+	DevBuf<TileRec> d_tiles;
 	unsigned tile_cap = 0;
-	unsigned* d_tile_tab = nullptr;
+	DevBuf<unsigned> d_tile_tab;
 	unsigned tile_tab_mask = 0;
-	unsigned* d_tile_n = nullptr;       // [0] tiles stored, [1] work counter, [2] new markers
-	uint8_t* d_tile_pool = nullptr;
+	DevBuf<unsigned> d_tile_n; // [0] tiles stored, [1] work counter, [2] new markers
+	DevBuf<uint8_t> d_tile_pool;
 	unsigned long long tile_pool_size = 0;
-	unsigned long long* d_tile_pool_top = nullptr;
-	unsigned long long* d_marker_set = nullptr;
+	DevBuf<unsigned long long> d_tile_pool_top;
+	DevBuf<unsigned long long> d_marker_set;
 	unsigned marker_set_mask = 0;
 	DevBuf<unsigned long long> new_markers, rep_tab, walk_dbg;
 	DevBuf<TileRec> tile_export;
@@ -1252,7 +1252,7 @@ struct abb_assembler {
 	// statistics
 	uint64_t st_iterations = 0, st_speculated = 0, st_wasted = 0, st_launches = 0, st_candidates = 0, st_contigs_tried = 0;
 	float ms_classify = 0, ms_visited = 0, ms_extend = 0, ms_replay = 0;
-	cudaEvent_t ev[2] = { nullptr, nullptr }, ev2[2] = { nullptr, nullptr };
+	Event ev[2], ev2[2];
 };
 
 namespace {
@@ -1289,13 +1289,10 @@ int ensure_scratch(abb_assembler* a, unsigned warps)
 
 int ensure_arena(abb_assembler* a, unsigned long long bytes)
 {
-	if (a->d_arena && a->arena_size >= bytes)
+	if (a->d_arena.p && a->arena_size >= bytes)
 		return ABB_OK;
-	if (a->d_arena)
-		cudaFree(a->d_arena);
-	a->d_arena = nullptr;
 	a->arena_size = 0;
-	ABB_CUDA(cudaMalloc((void**)&a->d_arena, bytes));
+	ABB_CHECK(a->d_arena.alloc(bytes)); // the old arena is freed first
 	a->arena_size = bytes;
 	return ABB_OK;
 }
@@ -1303,22 +1300,21 @@ int ensure_arena(abb_assembler* a, unsigned long long bytes)
 int ensure_endset(abb_assembler* a, uint64_t extra)
 {
 	const uint64_t need = (a->ends_upper + extra) * 2 + 16;
-	if (a->d_ends && need <= a->ends_cap)
+	if (a->d_ends.p && need <= a->ends_cap)
 		return ABB_OK;
 	uint64_t ncap = a->ends_cap ? a->ends_cap : 1024;
 	while (ncap < need)
 		ncap <<= 1;
 	ABB_REQUIRE(ncap <= (1ULL << 31), "contigEndKmers table too large");
-	unsigned long long* nt = nullptr;
-	ABB_CUDA(cudaMalloc((void**)&nt, ncap * sizeof(unsigned long long)));
-	ABB_CUDA(cudaMemsetAsync(nt, 0, ncap * sizeof(unsigned long long), a->stream));
-	if (a->d_ends) {
-		k_endset_rehash<<<256, 256, 0, a->stream>>>(a->d_ends, a->ends_cap, nt, (unsigned)ncap);
+	DevBuf<unsigned long long> nt;
+	ABB_CHECK(nt.alloc(ncap));
+	ABB_CUDA(cudaMemsetAsync(nt.p, 0, ncap * sizeof(unsigned long long), a->stream));
+	if (a->d_ends.p) {
+		k_endset_rehash<<<256, 256, 0, a->stream>>>(a->d_ends.p, a->ends_cap, nt.p, (unsigned)ncap);
 		ABB_CUDA(cudaGetLastError());
 		ABB_CUDA(cudaStreamSynchronize(a->stream));
-		cudaFree(a->d_ends);
 	}
-	a->d_ends = nt;
+	a->d_ends = std::move(nt); // frees the old table
 	a->ends_cap = (unsigned)ncap;
 	return ABB_OK;
 }
@@ -1330,7 +1326,7 @@ WalkCfg walk_cfg(const abb_assembler* a)
 	w.trim = a->params.trim;
 	w.threshold = a->solid->threshold;
 	w.rt = a->rt;
-	w.counters = a->solid->d_data;
+	w.counters = a->solid->d_data.p;
 	return w;
 }
 
@@ -1380,9 +1376,9 @@ int allgather_slices(abb_assembler* a, const uint8_t* mine, uint64_t n_total, ui
 TileView tile_view(const abb_assembler* a, bool on)
 {
 	TileView v = { nullptr, nullptr, 0 };
-	if (on && a->tiles_on && a->d_tile_tab) {
-		v.recs = a->d_tiles;
-		v.tab = a->d_tile_tab;
+	if (on && a->tiles_on && a->d_tile_tab.p) {
+		v.recs = a->d_tiles.p;
+		v.tab = a->d_tile_tab.p;
 		v.mask = a->tile_tab_mask;
 	}
 	return v;
@@ -1391,7 +1387,7 @@ TileView tile_view(const abb_assembler* a, bool on)
 /** allocate the tile store on first use, sized from the number of solid k-mers in the filter */
 int ensure_tile_store(abb_assembler* a)
 {
-	if (a->d_tile_tab || !a->tiles_on)
+	if (a->d_tile_tab.p || !a->tiles_on)
 		return ABB_OK;
 	uint64_t nz = 0, th = 0;
 	ABB_CHECK(abb_filter_popcount(a->solid, &nz, &th));
@@ -1399,27 +1395,39 @@ int ensure_tile_store(abb_assembler* a)
 	const uint64_t markers = solid / (kMarkerMask + 1) * 2 + 4096;
 	size_t free_b = 0, total_b = 0;
 	cudaMemGetInfo(&free_b, &total_b);
-	a->tile_cap = (unsigned)std::min<uint64_t>(markers * 4, 1u << 30);
+	const unsigned tile_cap = (unsigned)std::min<uint64_t>(markers * 4, 1u << 30);
 	unsigned long long pool = std::min<unsigned long long>(solid * 4 * 9 * 3 / 2 + (1 << 20), (unsigned long long)(free_b * 0.25));
 	uint64_t tab = 1;
-	while (tab < (uint64_t)a->tile_cap * 2)
+	while (tab < (uint64_t)tile_cap * 2)
 		tab <<= 1;
 	uint64_t mset = 1;
 	while (mset < markers * 4)
 		mset <<= 1;
-	ABB_CUDA(cudaMalloc((void**)&a->d_tiles, (size_t)a->tile_cap * sizeof(TileRec)));
-	ABB_CUDA(cudaMalloc((void**)&a->d_tile_tab, tab * sizeof(unsigned)));
-	ABB_CUDA(cudaMemsetAsync(a->d_tile_tab, 0, tab * sizeof(unsigned), a->stream));
+	// the store takes the six pieces only once all of them exist: a store with d_tile_tab set counts as complete
+	DevBuf<TileRec> tiles;
+	DevBuf<unsigned> tile_tab, tile_n;
+	DevBuf<unsigned long long> marker_set, pool_top;
+	DevBuf<uint8_t> tile_pool;
+	ABB_CHECK(tiles.alloc(tile_cap));
+	ABB_CHECK(tile_tab.alloc(tab));
+	ABB_CUDA(cudaMemsetAsync(tile_tab.p, 0, tab * sizeof(unsigned), a->stream));
+	ABB_CHECK(marker_set.alloc(mset));
+	ABB_CUDA(cudaMemsetAsync(marker_set.p, 0, mset * sizeof(unsigned long long), a->stream));
+	ABB_CHECK(tile_pool.alloc(pool));
+	ABB_CHECK(tile_n.alloc(4));
+	ABB_CUDA(cudaMemsetAsync(tile_n.p, 0, 4 * sizeof(unsigned), a->stream));
+	ABB_CHECK(pool_top.alloc(1));
+	ABB_CUDA(cudaMemsetAsync(pool_top.p, 0, sizeof(unsigned long long), a->stream));
+	a->d_tiles = std::move(tiles);
+	a->tile_cap = tile_cap;
+	a->d_tile_tab = std::move(tile_tab);
 	a->tile_tab_mask = (unsigned)(tab - 1);
-	ABB_CUDA(cudaMalloc((void**)&a->d_marker_set, mset * sizeof(unsigned long long)));
-	ABB_CUDA(cudaMemsetAsync(a->d_marker_set, 0, mset * sizeof(unsigned long long), a->stream));
+	a->d_marker_set = std::move(marker_set);
 	a->marker_set_mask = (unsigned)(mset - 1);
-	ABB_CUDA(cudaMalloc((void**)&a->d_tile_pool, pool));
+	a->d_tile_pool = std::move(tile_pool);
 	a->tile_pool_size = pool;
-	ABB_CUDA(cudaMalloc((void**)&a->d_tile_n, 4 * sizeof(unsigned)));
-	ABB_CUDA(cudaMemsetAsync(a->d_tile_n, 0, 4 * sizeof(unsigned), a->stream));
-	ABB_CUDA(cudaMalloc((void**)&a->d_tile_pool_top, sizeof(unsigned long long)));
-	ABB_CUDA(cudaMemsetAsync(a->d_tile_pool_top, 0, sizeof(unsigned long long), a->stream));
+	a->d_tile_n = std::move(tile_n);
+	a->d_tile_pool_top = std::move(pool_top);
 	return ABB_OK;
 }
 
@@ -1454,20 +1462,20 @@ int exchange_tiles(abb_assembler* a, unsigned n0, unsigned n1, unsigned long lon
 	// 3. my records with pool-relative pointers, then the two exchanges
 	ABB_CHECK(a->tile_export.reserve((size_t)(n1 - n0) + 1));
 	if (n1 > n0)
-		k_export_tiles<<<blocks_for(n1 - n0, 256), 256, 0, st>>>(a->d_tiles, n0, n1 - n0, a->d_tile_pool + p0, a->tile_export.p);
+		k_export_tiles<<<blocks_for(n1 - n0, 256), 256, 0, st>>>(a->d_tiles.p, n0, n1 - n0, a->d_tile_pool.p + p0, a->tile_export.p);
 	ABB_CUDA(cudaGetLastError());
-	ABB_CHECK(abb_comm_exchange_bytes(a->comm, a->tile_export.p, (uint64_t)(n1 - n0) * sizeof(TileRec), a->d_tiles, rec_off.data(), rec_bytes.data(), st));
-	ABB_CHECK(abb_comm_exchange_bytes(a->comm, a->d_tile_pool + p0, p1 - p0, a->d_tile_pool, pool_off.data(), pool_bytes.data(), st));
+	ABB_CHECK(abb_comm_exchange_bytes(a->comm, a->tile_export.p, (uint64_t)(n1 - n0) * sizeof(TileRec), a->d_tiles.p, rec_off.data(), rec_bytes.data(), st));
+	ABB_CHECK(abb_comm_exchange_bytes(a->comm, a->d_tile_pool.p + p0, p1 - p0, a->d_tile_pool.p, pool_off.data(), pool_bytes.data(), st));
 	for (unsigned r = 0; r < world; ++r) {
 		if (r == rank || all[2 * r] == 0)
 			continue;
 		const unsigned first = (unsigned)(rec_off[r] / sizeof(TileRec)), n = (unsigned)all[2 * r];
-		k_import_tiles<<<blocks_for(n, 256), 256, 0, st>>>(a->d_tiles, first, n, a->d_tile_pool + pool_off[r], a->d_tile_tab, a->tile_tab_mask);
+		k_import_tiles<<<blocks_for(n, 256), 256, 0, st>>>(a->d_tiles.p, first, n, a->d_tile_pool.p + pool_off[r], a->d_tile_tab.p, a->tile_tab_mask);
 	}
 	ABB_CUDA(cudaGetLastError());
 	const unsigned nt32 = (unsigned)nt;
-	ABB_CUDA(cudaMemcpyAsync(a->d_tile_n, &nt32, sizeof nt32, cudaMemcpyHostToDevice, st));
-	ABB_CUDA(cudaMemcpyAsync(a->d_tile_pool_top, &pt, sizeof pt, cudaMemcpyHostToDevice, st));
+	ABB_CUDA(cudaMemcpyAsync(a->d_tile_n.p, &nt32, sizeof nt32, cudaMemcpyHostToDevice, st));
+	ABB_CUDA(cudaMemcpyAsync(a->d_tile_pool_top.p, &pt, sizeof pt, cudaMemcpyHostToDevice, st));
 	ABB_CUDA(cudaStreamSynchronize(st));
 	a->st_launches += 2 + world;
 	return ABB_OK;
@@ -1486,15 +1494,15 @@ int produce_tiles(abb_assembler* a, uint64_t n_reads, uint64_t n_slots)
 	const unsigned world = a->comm ? (unsigned)abb_comm_world(a->comm) : 1u, rank = a->comm ? (unsigned)abb_comm_rank(a->comm) : 0u;
 	const unsigned out_cap = (unsigned)std::min<uint64_t>(n_slots / (kMarkerMask + 1) * 2 + 4096, a->marker_set_mask / 2 + 1);
 	ABB_CHECK(a->new_markers.reserve(out_cap));
-	ABB_CUDA(cudaMemsetAsync(a->d_tile_n + 1, 0, 2 * sizeof(unsigned), st));
-	k_find_markers<<<sm_count() * 16, 256, 0, st>>>(a->h0.p, a->valid.p, a->slot_offs.p, n_reads, n_slots, w, f->cfg, a->d_marker_set,
-	                                         a->marker_set_mask, a->new_markers.p, a->d_tile_n + 2, out_cap, world, rank);
+	ABB_CUDA(cudaMemsetAsync(a->d_tile_n.p + 1, 0, 2 * sizeof(unsigned), st));
+	k_find_markers<<<sm_count() * 16, 256, 0, st>>>(a->h0.p, a->valid.p, a->slot_offs.p, n_reads, n_slots, w, f->cfg, a->d_marker_set.p,
+	                                         a->marker_set_mask, a->new_markers.p, a->d_tile_n.p + 2, out_cap, world, rank);
 	ABB_CUDA(cudaGetLastError());
 	unsigned nm = 0, n0 = 0;
 	unsigned long long p0 = 0;
-	ABB_CUDA(cudaMemcpyAsync(&nm, a->d_tile_n + 2, sizeof nm, cudaMemcpyDeviceToHost, st));
-	ABB_CUDA(cudaMemcpyAsync(&n0, a->d_tile_n, sizeof n0, cudaMemcpyDeviceToHost, st));
-	ABB_CUDA(cudaMemcpyAsync(&p0, a->d_tile_pool_top, sizeof p0, cudaMemcpyDeviceToHost, st));
+	ABB_CUDA(cudaMemcpyAsync(&nm, a->d_tile_n.p + 2, sizeof nm, cudaMemcpyDeviceToHost, st));
+	ABB_CUDA(cudaMemcpyAsync(&n0, a->d_tile_n.p, sizeof n0, cudaMemcpyDeviceToHost, st));
+	ABB_CUDA(cudaMemcpyAsync(&p0, a->d_tile_pool_top.p, sizeof p0, cudaMemcpyDeviceToHost, st));
 	ABB_CUDA(cudaStreamSynchronize(st));
 	nm = std::min(nm, out_cap);
 	n0 = std::min(n0, a->tile_cap);
@@ -1518,18 +1526,18 @@ int produce_tiles(abb_assembler* a, uint64_t n_reads, uint64_t n_slots)
 		ABB_CHECK(ensure_scratch(a, warps));
 		ABB_CHECK(a->stage_bases.reserve((size_t)warps * kTileCap));
 		ABB_CHECK(a->stage_hashes.reserve((size_t)warps * kTileCap));
-		TileStore ts = { a->d_tiles, a->d_tile_tab, a->tile_tab_mask, a->tile_cap, a->d_tile_n, a->d_tile_pool, a->tile_pool_size,
-			             a->d_tile_pool_top };
+		TileStore ts = { a->d_tiles.p, a->d_tile_tab.p, a->tile_tab_mask, a->tile_cap, a->d_tile_n.p, a->d_tile_pool.p, a->tile_pool_size,
+			             a->d_tile_pool_top.p };
 		ABB_DISPATCH_KW(a->kw, (k_make_tiles<KW><<<grid, kWalkWarps * 32, 0, st>>>(a->cur_bases, a->cur_offs, a->new_markers.p, nm,
-		                                                                          a->d_tile_n + 1, w, f->cfg, a->frames.p, a->look.p,
+		                                                                          a->d_tile_n.p + 1, w, f->cfg, a->frames.p, a->look.p,
 		                                                                          a->stage_bases.p, a->stage_hashes.p, ts)));
 		ABB_CUDA(cudaGetLastError());
 		a->st_launches += 1;
 	}
 	unsigned nt = 0;
 	unsigned long long p1 = 0;
-	ABB_CUDA(cudaMemcpyAsync(&nt, a->d_tile_n, sizeof nt, cudaMemcpyDeviceToHost, st));
-	ABB_CUDA(cudaMemcpyAsync(&p1, a->d_tile_pool_top, sizeof p1, cudaMemcpyDeviceToHost, st));
+	ABB_CUDA(cudaMemcpyAsync(&nt, a->d_tile_n.p, sizeof nt, cudaMemcpyDeviceToHost, st));
+	ABB_CUDA(cudaMemcpyAsync(&p1, a->d_tile_pool_top.p, sizeof p1, cudaMemcpyDeviceToHost, st));
 	ABB_CUDA(cudaStreamSynchronize(st));
 	nt = std::min(nt, a->tile_cap);
 	p1 = std::min(p1, a->tile_pool_size);
@@ -1537,11 +1545,11 @@ int produce_tiles(abb_assembler* a, uint64_t n_reads, uint64_t n_slots)
 	a->st_tiles = nt;
 	if (world > 1) {
 		ABB_CHECK(exchange_tiles(a, n0, nt, p0, p1));
-		ABB_CUDA(cudaMemcpyAsync(&nt, a->d_tile_n, sizeof nt, cudaMemcpyDeviceToHost, st));
+		ABB_CUDA(cudaMemcpyAsync(&nt, a->d_tile_n.p, sizeof nt, cudaMemcpyDeviceToHost, st));
 		ABB_CUDA(cudaStreamSynchronize(st));
 		a->st_tiles = nt;
 	}
-	k_link_tiles<<<sm_count() * 8, 256, 0, st>>>(a->d_tiles, (unsigned)a->st_tiles, a->d_tile_tab, a->tile_tab_mask);
+	k_link_tiles<<<sm_count() * 8, 256, 0, st>>>(a->d_tiles.p, (unsigned)a->st_tiles, a->d_tile_tab.p, a->tile_tab_mask);
 	ABB_CUDA(cudaGetLastError());
 	a->st_launches += 1;
 	tt.stop();
@@ -1561,7 +1569,7 @@ int run_extend(abb_assembler* a, unsigned n_spec, bool use_tiles, bool keep_aren
 	status.assign(n_spec, 0);
 	unsigned long long arena_mark = 0;
 	if (keep_arena) {
-		ABB_CUDA(cudaMemcpyAsync(&arena_mark, a->d_arena_top, sizeof arena_mark, cudaMemcpyDeviceToHost, st));
+		ABB_CUDA(cudaMemcpyAsync(&arena_mark, a->d_arena_top.p, sizeof arena_mark, cudaMemcpyDeviceToHost, st));
 		ABB_CUDA(cudaStreamSynchronize(st));
 	}
 	for (;;) {
@@ -1573,19 +1581,19 @@ int run_extend(abb_assembler* a, unsigned n_spec, bool use_tiles, bool keep_aren
 			dbg = a->walk_dbg.p;
 		}
 		ABB_CHECK(ensure_arena(a, a->arena_size ? a->arena_size : std::max(kArenaDefault, g_arena_hint)));
-		ABB_CUDA(cudaMemcpyAsync(a->d_arena_top, &arena_mark, sizeof arena_mark, cudaMemcpyHostToDevice, st));
-		ABB_CUDA(cudaMemsetAsync(a->d_nrecs, 0, sizeof(unsigned), st));
+		ABB_CUDA(cudaMemcpyAsync(a->d_arena_top.p, &arena_mark, sizeof arena_mark, cudaMemcpyHostToDevice, st));
+		ABB_CUDA(cudaMemsetAsync(a->d_nrecs.p, 0, sizeof(unsigned), st));
 		const WalkCfg w = walk_cfg(a);
 		const TileView tv = tile_view(a, use_tiles);
 		cudaEventRecord(a->ev2[0], st);
 		ABB_DISPATCH_KW(a->kw, (k_extend<KW><<<blocks_for(n_spec, kWalkWarps), kWalkWarps * 32, 0, st>>>(
-		                           a->cur_bases, a->cur_offs, a->spec.p, n_spec, w, f->cfg, a->frames.p, a->look.p, a->d_arena, a->arena_size,
-		                           a->d_arena_top, a->recs.p, a->d_nrecs, rec_cap, a->status.p, tv, dbg)));
+		                           a->cur_bases, a->cur_offs, a->spec.p, n_spec, w, f->cfg, a->frames.p, a->look.p, a->d_arena.p, a->arena_size,
+		                           a->d_arena_top.p, a->recs.p, a->d_nrecs.p, rec_cap, a->status.p, tv, dbg)));
 		ABB_CUDA(cudaGetLastError());
 		cudaEventRecord(a->ev2[1], st);
 		++a->st_launches;
 		unsigned nrecs = 0;
-		ABB_CUDA(cudaMemcpyAsync(&nrecs, a->d_nrecs, sizeof nrecs, cudaMemcpyDeviceToHost, st));
+		ABB_CUDA(cudaMemcpyAsync(&nrecs, a->d_nrecs.p, sizeof nrecs, cudaMemcpyDeviceToHost, st));
 		ABB_CUDA(cudaMemcpyAsync(status.data(), a->status.p, n_spec * sizeof(unsigned), cudaMemcpyDeviceToHost, st));
 		ABB_CUDA(cudaStreamSynchronize(st));
 		{
@@ -1699,7 +1707,7 @@ int stage_contigs(abb_assembler* a, const std::vector<ContigRec>& recs, const Ro
 		k_gather<<<std::min<unsigned>(ns, sm_count() * 16), 256, 0, st>>>(a->recs_sorted.p, a->seg_contig.p, a->seg_beg.p, a->seg_len.p, ns, a->coffs.p,
 		                                                          a->cseq.p, f->k, a->rt);
 		ABB_CUDA(cudaGetLastError());
-		ABB_CHECK(launch_hash_segments(f->k, f->d_care, a->cseq.p, a->seg_beg.p, a->seg_len.p, a->seg_slot.p, ns, a->ch0.p, a->cvalid.p, st));
+		ABB_CHECK(launch_hash_segments(f->k, f->d_care.p, a->cseq.p, a->seg_beg.p, a->seg_len.p, a->seg_slot.p, ns, a->ch0.p, a->cvalid.p, st));
 		cudaEventRecord(a->ev2[1], st);
 		cudaEventSynchronize(a->ev2[1]);
 		float ms = 0;
@@ -1730,7 +1738,7 @@ int speculate_round(abb_assembler* a, const std::vector<unsigned>& cand, size_t*
 			const unsigned vlo = (unsigned)((uint64_t)rank * n / world), vup = (unsigned)((uint64_t)(rank + 1) * n / world);
 			if (vup > vlo)
 				k_visited<<<blocks_for((uint64_t)(vup - vlo) * 32, 256), 256, 0, st>>>(a->cand.p, (unsigned)pos + vlo, vup - vlo, a->slot_offs.p, a->h0.p,
-				                                                                      f->cfg, a->assembled->d_data, a->vis.p + vlo);
+				                                                                      f->cfg, a->assembled->d_data.p, a->vis.p + vlo);
 			ABB_CUDA(cudaGetLastError());
 			++a->st_launches;
 			if (world > 1)
@@ -1790,7 +1798,7 @@ int speculate_round(abb_assembler* a, const std::vector<unsigned>& cand, size_t*
 			return ABB_ENOMEM;
 		}
 		// repeat check on everything that was produced with tiles
-		if (a->tiles_on && a->d_tile_tab) {
+		if (a->tiles_on && a->d_tile_tab.p) {
 			std::vector<ContigRec> keep;
 			for (auto& r : recs)
 				if (r.spec < n_ok && std::find(redo.begin(), redo.end(), r.spec) == redo.end())
@@ -1905,11 +1913,11 @@ int speculate_round(abb_assembler* a, const std::vector<unsigned>& cand, size_t*
 		io.clen = a->clen.p;
 		io.cseq = a->cseq.p;
 		io.coffs = a->coffs.p;
-		io.care = a->solid->d_care;
+		io.care = a->solid->d_care.p;
 		io.rcode = a->rcode.p;
 		io.caccept = a->caccept.p;
 		io.ccov = a->ccov.p;
-		EndSet ends = { a->d_ends, a->ends_cap, a->d_ends_n };
+		EndSet ends = { a->d_ends.p, a->ends_cap, a->d_ends_n.p };
 		if (nc) {
 			ABB_CUDA(cudaMemsetAsync(a->caccept.p, 0, nc, st));
 			ABB_CUDA(cudaMemsetAsync(a->ccov.p, 0, nc * sizeof(unsigned), st));
@@ -1938,8 +1946,8 @@ int speculate_round(abb_assembler* a, const std::vector<unsigned>& cand, size_t*
 			unsigned n_big = (unsigned)big.size(), nc_arg = nc, k_arg = f->k;
 			const unsigned* d_big = a->big_idx.p;
 			const unsigned* d_big_s = a->big_spec.p;
-			const uint8_t* d_counters = f->d_data;
-			uint8_t* d_bits = a->assembled->d_data;
+			const uint8_t* d_counters = f->d_data.p;
+			uint8_t* d_bits = a->assembled->d_data.p;
 			void* params[] = { &io, &nc_arg, &d_big, &d_big_s, &n_big, &f->cfg, &k_arg, &d_counters, &d_bits, &ends };
 			ABB_CUDA(cudaLaunchCooperativeKernel((void*)k_replay_all, dim3((unsigned)replay_grid), dim3(1024), params, 0, st));
 			++a->st_launches;
@@ -2043,7 +2051,7 @@ int abb_assembler_create(abb_assembler** out, abb_filter* solid, const abb_assem
 	}
 	ABB_REQUIRE(solid->k >= 2, "k must be at least 2 for graph traversal");
 	ABB_CUDA(cudaSetDevice(solid->device));
-	abb_assembler* a = new (std::nothrow) abb_assembler();
+	std::unique_ptr<abb_assembler> a(new (std::nothrow) abb_assembler());
 	if (!a) {
 		set_error("out of host memory");
 		return ABB_ENOMEM;
@@ -2060,14 +2068,13 @@ int abb_assembler_create(abb_assembler** out, abb_filter* solid, const abb_assem
 			if (solid->mask[i] == '0')
 				mpos.push_back((uint8_t)i);
 		if (!mpos.empty()) {
-			if (cudaMalloc((void**)&a->d_mpos, mpos.size()) != cudaSuccess ||
-			    cudaMemcpy(a->d_mpos, mpos.data(), mpos.size(), cudaMemcpyHostToDevice) != cudaSuccess) {
+			if (a->d_mpos.alloc(mpos.size()) != ABB_OK ||
+			    cudaMemcpy(a->d_mpos.p, mpos.data(), mpos.size(), cudaMemcpyHostToDevice) != cudaSuccess) {
 				set_error("cudaMalloc of the spaced-seed table failed");
-				delete a;
 				return ABB_ECUDA;
 			}
 			a->rt.nmask = (unsigned)mpos.size();
-			a->rt.mpos = a->d_mpos;
+			a->rt.mpos = a->d_mpos.p;
 		}
 	}
 	// tiles are keyed by vertex hash and assume that equal hashes continue identically; with a spaced seed two k-mers
@@ -2076,68 +2083,25 @@ int abb_assembler_create(abb_assembler** out, abb_filter* solid, const abb_assem
 	if (const char* sp = getenv("ABB_SPEC")) // tuning switch: fixed speculation width
 		a->spec_fixed = a->spec_target = (unsigned)std::max(1, atoi(sp));
 	// BloomFilter assembledKmerSet(solid.size(), solid.getHashNum(), solid.getKmerSize()) (bloom-dbg.h:910-911)
-	int rc = abb_filter_create(&a->assembled, ABB_BIT, solid->size, solid->H, solid->k, 0, "", solid->device);
-	if (rc != ABB_OK) {
-		delete a;
-		return rc;
-	}
-	auto fail = [&](cudaError_t e, const char* what) {
-		set_error("%s: %s", what, cudaGetErrorString(e));
-		abb_assembler_destroy(a);
-		return e == cudaErrorMemoryAllocation ? ABB_ENOMEM : ABB_ECUDA;
-	};
-	cudaError_t e;
+	abb_filter* assembled = nullptr;
+	ABB_CHECK(abb_filter_create(&assembled, ABB_BIT, solid->size, solid->H, solid->k, 0, "", solid->device));
+	a->assembled.reset(assembled);
 	a->stream = solid->stream; // one stream carries pass 1 and pass 2 of a filter
-	if ((e = cudaEventCreate(&a->ev[0])) != cudaSuccess) return fail(e, "cudaEventCreate");
-	if ((e = cudaEventCreate(&a->ev[1])) != cudaSuccess) return fail(e, "cudaEventCreate");
-	if ((e = cudaEventCreate(&a->ev2[0])) != cudaSuccess) return fail(e, "cudaEventCreate");
-	if ((e = cudaEventCreate(&a->ev2[1])) != cudaSuccess) return fail(e, "cudaEventCreate");
-	if ((e = cudaMalloc((void**)&a->d_arena_top, sizeof(unsigned long long))) != cudaSuccess) return fail(e, "cudaMalloc");
-	if ((e = cudaMalloc((void**)&a->d_nrecs, sizeof(unsigned))) != cudaSuccess) return fail(e, "cudaMalloc");
-	if ((e = cudaMalloc((void**)&a->d_ends_n, 2 * sizeof(unsigned))) != cudaSuccess) return fail(e, "cudaMalloc");
-	if ((e = cudaMemset(a->d_ends_n, 0, 2 * sizeof(unsigned))) != cudaSuccess) return fail(e, "cudaMemset");
-	*out = a;
-	return ABB_OK;
+	for (Event* e : { &a->ev[0], &a->ev[1], &a->ev2[0], &a->ev2[1] })
+		ABB_CUDA(cudaEventCreate(e->out()));
+	ABB_CHECK(a->d_arena_top.alloc(1));
+	ABB_CHECK(a->d_nrecs.alloc(1));
+	ABB_CHECK(a->d_ends_n.alloc(2));
+	ABB_CUDA(cudaMemset(a->d_ends_n.p, 0, 2 * sizeof(unsigned)));
+	return hand_over(a, out);
 }
 
 int abb_assembler_destroy(abb_assembler* a)
 {
 	if (!a)
 		return ABB_OK;
-	if (a->solid)
-		cudaSetDevice(a->solid->device);
-	if (a->stream)
-		cudaStreamSynchronize(a->stream);
-	abb_filter_destroy(a->assembled);
-	a->bases.release(); a->valid.release(); a->codes.release(); a->vis.release(); a->scan_tmp.release();
-	a->cseq.release(); a->cvalid.release(); a->rcode.release(); a->caccept.release();
-	a->offs.release(); a->slot_offs.release(); a->h0.release(); a->coffs.release(); a->cslot.release(); a->ch0.release();
-	a->cand.release(); a->spec.release(); a->spec_cbeg.release(); a->clen.release(); a->ccov.release(); a->status.release();
-	a->recs.release(); a->recs_sorted.release(); a->frames.release(); a->look.release();
-	cudaFree(a->d_mpos);
-	cudaFree(a->d_tiles);
-	cudaFree(a->d_tile_tab);
-	cudaFree(a->d_tile_n);
-	cudaFree(a->d_tile_pool);
-	cudaFree(a->d_tile_pool_top);
-	cudaFree(a->d_marker_set);
-	a->rep_off.release();
-	a->gather.release();
-	a->walk_dbg.release();
-	a->big_idx.release();
-	a->big_spec.release();
-	a->tile_export.release();
-	a->seg_contig.release(); a->seg_len.release(); a->seg_beg.release(); a->seg_slot.release();
-	a->new_markers.release(); a->rep_tab.release(); a->stage_bases.release(); a->rep_flag.release(); a->stage_hashes.release();
-	cudaFree(a->d_arena);
-	cudaFree(a->d_arena_top);
-	cudaFree(a->d_nrecs);
-	cudaFree(a->d_ends);
-	cudaFree(a->d_ends_n);
-	if (a->ev[0]) cudaEventDestroy(a->ev[0]);
-	if (a->ev[1]) cudaEventDestroy(a->ev[1]);
-	if (a->ev2[0]) cudaEventDestroy(a->ev2[0]);
-	if (a->ev2[1]) cudaEventDestroy(a->ev2[1]);
+	cudaSetDevice(a->solid->device);
+	cudaStreamSynchronize(a->stream);
 	delete a;
 	return ABB_OK;
 }
@@ -2154,7 +2118,7 @@ static int hash_and_classify(abb_assembler* a, const uint8_t* d_bases, const uin
 	ABB_CHECK(a->valid.reserve(total + 1));
 	ABB_CHECK(a->codes.reserve(n_reads));
 	if (total)
-		ABB_CHECK(launch_hash(nullptr, f->k, f->d_care, d_bases, d_offs, a->slot_offs.p, 0, n_reads, 0, a->h0.p, a->valid.p, st,
+		ABB_CHECK(launch_hash(nullptr, f->k, f->d_care.p, d_bases, d_offs, a->slot_offs.p, 0, n_reads, 0, a->h0.p, a->valid.p, st,
 		                      &a->st_launches));
 	*total_out = total;
 	if (!classify)
@@ -2214,11 +2178,11 @@ static int process_batch(abb_assembler* a, const uint8_t* d_bases, const uint64_
 		IsCandidate pred{ a->codes.p };
 		thrust::counting_iterator<unsigned> first(0);
 		size_t bytes = 0;
-		ABB_CUDA(cub::DeviceSelect::If(nullptr, bytes, first, a->cand.p, a->d_nrecs, (int)n_reads, pred, st));
+		ABB_CUDA(cub::DeviceSelect::If(nullptr, bytes, first, a->cand.p, a->d_nrecs.p, (int)n_reads, pred, st));
 		ABB_CHECK(a->scan_tmp.reserve(bytes));
-		ABB_CUDA(cub::DeviceSelect::If(a->scan_tmp.p, bytes, first, a->cand.p, a->d_nrecs, (int)n_reads, pred, st));
+		ABB_CUDA(cub::DeviceSelect::If(a->scan_tmp.p, bytes, first, a->cand.p, a->d_nrecs.p, (int)n_reads, pred, st));
 		unsigned nc = 0;
-		ABB_CUDA(cudaMemcpyAsync(&nc, a->d_nrecs, sizeof nc, cudaMemcpyDeviceToHost, st));
+		ABB_CUDA(cudaMemcpyAsync(&nc, a->d_nrecs.p, sizeof nc, cudaMemcpyDeviceToHost, st));
 		ABB_CUDA(cudaStreamSynchronize(st));
 		cand.resize(nc);
 		if (nc)
@@ -2343,16 +2307,16 @@ int abb_assembler_reset(abb_assembler* a)
 	ABB_CUDA(cudaSetDevice(a->solid->device));
 	cudaStream_t st = a->stream;
 	ABB_CUDA(cudaStreamSynchronize(st));
-	ABB_CHECK(abb_filter_clear(a->assembled));
-	if (a->d_ends)
-		ABB_CUDA(cudaMemsetAsync(a->d_ends, 0, (size_t)a->ends_cap * sizeof(unsigned long long), st));
-	ABB_CUDA(cudaMemsetAsync(a->d_ends_n, 0, 2 * sizeof(unsigned), st));
+	ABB_CHECK(abb_filter_clear(a->assembled.get()));
+	if (a->d_ends.p)
+		ABB_CUDA(cudaMemsetAsync(a->d_ends.p, 0, (size_t)a->ends_cap * sizeof(unsigned long long), st));
+	ABB_CUDA(cudaMemsetAsync(a->d_ends_n.p, 0, 2 * sizeof(unsigned), st));
 	a->ends_upper = 0;
-	if (a->d_tile_tab) { // the tiles describe the old contents of the solid filter: forget them, keep the memory
-		ABB_CUDA(cudaMemsetAsync(a->d_tile_tab, 0, ((size_t)a->tile_tab_mask + 1) * sizeof(unsigned), st));
-		ABB_CUDA(cudaMemsetAsync(a->d_marker_set, 0, ((size_t)a->marker_set_mask + 1) * sizeof(unsigned long long), st));
-		ABB_CUDA(cudaMemsetAsync(a->d_tile_n, 0, 4 * sizeof(unsigned), st));
-		ABB_CUDA(cudaMemsetAsync(a->d_tile_pool_top, 0, sizeof(unsigned long long), st));
+	if (a->d_tile_tab.p) { // the tiles describe the old contents of the solid filter: forget them, keep the memory
+		ABB_CUDA(cudaMemsetAsync(a->d_tile_tab.p, 0, ((size_t)a->tile_tab_mask + 1) * sizeof(unsigned), st));
+		ABB_CUDA(cudaMemsetAsync(a->d_marker_set.p, 0, ((size_t)a->marker_set_mask + 1) * sizeof(unsigned long long), st));
+		ABB_CUDA(cudaMemsetAsync(a->d_tile_n.p, 0, 4 * sizeof(unsigned), st));
+		ABB_CUDA(cudaMemsetAsync(a->d_tile_pool_top.p, 0, sizeof(unsigned long long), st));
 	}
 	ABB_CUDA(cudaStreamSynchronize(st));
 	a->counters = abb_assembly_counters{};
@@ -2405,6 +2369,6 @@ int abb_assembler_read_results(const abb_assembler* a, const uint8_t** codes, ui
 	return ABB_OK;
 }
 
-abb_filter* abb_assembler_assembled_filter(abb_assembler* a) { return a ? a->assembled : nullptr; }
+abb_filter* abb_assembler_assembled_filter(abb_assembler* a) { return a ? a->assembled.get() : nullptr; }
 
 } // extern "C"

@@ -5,7 +5,9 @@
 #include <cuda_runtime.h>
 #include <cstdarg>
 #include <cstdio>
+#include <memory>
 #include <string>
+#include <utility>
 #include <vector>
 
 namespace abb {
@@ -16,6 +18,7 @@ void set_error(const char* fmt, ...);
 	do {                                                                                           \
 		cudaError_t e__ = (call);                                                                  \
 		if (e__ != cudaSuccess) {                                                                  \
+			cudaGetLastError(); /* returned here: a later launch check must not report it again */ \
 			abb::set_error("%s:%d: %s failed: %s", __FILE__, __LINE__, #call, cudaGetErrorString(e__)); \
 			return (e__ == cudaErrorMemoryAllocation) ? ABB_ENOMEM                                 \
 			       : (e__ == cudaErrorNoDevice || e__ == cudaErrorInsufficientDriver) ? ABB_ENODEV \
@@ -47,25 +50,35 @@ void set_error(const char* fmt, ...);
 		}                                                                                           \
 	} while (0)
 
-/** growable device buffer */
+/** Device buffer that owns its allocation: freed by the destructor, moved but never copied.  Every owner lives in a
+ *  handle or on the stack of a C-ABI call, never in static storage (its destructor would run after the runtime shut down). */
 template <typename T>
 struct DevBuf {
 	T* p = nullptr;
 	size_t cap = 0;
-	int reserve(size_t n)
+	DevBuf() = default;
+	DevBuf(DevBuf&& o) noexcept { *this = std::move(o); }
+	DevBuf& operator=(DevBuf&& o) noexcept
 	{
-		if (n <= cap)
-			return ABB_OK;
-		if (p)
-			cudaFree(p);
-		p = nullptr;
-		cap = 0;
-		size_t want = n + n / 8 + 256;
-		ABB_CUDA(cudaMalloc((void**)&p, want * sizeof(T)));
-		cap = want;
+		if (this != &o) {
+			reset();
+			std::swap(p, o.p);
+			std::swap(cap, o.cap);
+		}
+		return *this;
+	}
+	~DevBuf() { reset(); }
+	/** at least n elements, with slack for growing batches; the contents are not kept */
+	int reserve(size_t n) { return n <= cap ? ABB_OK : alloc(n + n / 8 + 256); }
+	/** exactly n elements, the old allocation freed first (peak memory); the contents are not kept */
+	int alloc(size_t n)
+	{
+		reset();
+		ABB_CUDA(cudaMalloc((void**)&p, n * sizeof(T)));
+		cap = n;
 		return ABB_OK;
 	}
-	void release()
+	void reset()
 	{
 		if (p)
 			cudaFree(p);
@@ -73,6 +86,45 @@ struct DevBuf {
 		cap = 0;
 	}
 };
+
+/** A CUDA stream or event owned like DevBuf; it converts to the raw handle for the runtime calls that use it. */
+template <typename H, cudaError_t (*Destroy)(H)>
+struct Owned {
+	H h = nullptr;
+	Owned() = default;
+	Owned(Owned&& o) noexcept { std::swap(h, o.h); }
+	~Owned() { reset(); }
+	operator H() const { return h; }
+	/** for the create call: destroys the current handle and hands out the slot for the new one */
+	H* out()
+	{
+		reset();
+		return &h;
+	}
+	void reset()
+	{
+		if (h)
+			Destroy(h);
+		h = nullptr;
+	}
+};
+using Stream = Owned<cudaStream_t, cudaStreamDestroy>;
+using Event = Owned<cudaEvent_t, cudaEventDestroy>;
+
+/** synchronises the stream when the scope ends, on every return path: no asynchronous copy into a caller's buffer
+ *  outlives the C-ABI call that queued it */
+struct SyncOnExit {
+	cudaStream_t s;
+	~SyncOnExit() { cudaStreamSynchronize(s); }
+};
+
+/** hands a finished handle to the C caller, whose abb_*_destroy owns it from then on */
+template <typename T>
+int hand_over(std::unique_ptr<T>& h, T** out)
+{
+	*out = h.release();
+	return ABB_OK;
+}
 
 inline unsigned blocks_for(uint64_t n, unsigned threads) { return (unsigned)((n + threads - 1) / threads); }
 
@@ -116,14 +168,14 @@ struct abb_filter {
 	unsigned H = 0, k = 0, threshold = 0, levels = 1;
 	uint64_t kon_full = 0, kon_start = 0, kon_seed = 0; // ABB_KONNECTOR: filter size in bits, first bit held, hash seed
 	std::string mask;
-	uint8_t* d_care = nullptr; // k bytes (mask == '1'), only with a spaced seed
-	uint8_t* d_data = nullptr;
+	abb::DevBuf<uint8_t> d_care; // k bytes (mask == '1'), only with a spaced seed
+	abb::DevBuf<uint8_t> d_data;
 	abb::HashCfg cfg;
-	cudaStream_t stream = nullptr;
-	cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+	abb::Stream stream;
+	abb::Event ev0, ev1;
 	// host-buffer insert: the bases travel in pieces on their own stream while earlier chunks are hashed and inserted
-	cudaStream_t copy_stream = nullptr;
-	std::vector<cudaEvent_t> copy_ev; // copy_ev[i]: piece i has landed
+	abb::Stream copy_stream;
+	std::vector<abb::Event> copy_ev; // copy_ev[i]: piece i has landed
 
 	// ordered-insert workspace (abb_insert.cuh K2)
 	uint64_t window = 0;      // slots per window
@@ -131,14 +183,15 @@ struct abb_filter {
 	unsigned ws_H = 0;
 	uint64_t map_entries = 0; // two-bit entries per conflict map (power of two)
 	unsigned map_log2 = 0;    // 0 = default size
-	unsigned* d_map[3] = { nullptr, nullptr, nullptr }; // one allocation
-	unsigned long long* d_tags2[2] = { nullptr, nullptr }; // tag tables of the carried slots (alternating windows)
+	abb::DevBuf<unsigned> maps;                         // the three maps in one allocation (one L2 access-policy window covers them)
+	unsigned* d_map[3] = { nullptr, nullptr, nullptr }; // the maps within `maps`
+	abb::DevBuf<unsigned long long> d_tags2[2];         // tag tables of the carried slots (alternating windows)
 	uint64_t tag_slots = 0;
-	uint64_t* d_carry = nullptr;    // two carry lists and the drain's sorted list, (window + kCarryLanes) slots each
-	unsigned* d_slotbits = nullptr; // presence bitmap of the drain
+	abb::DevBuf<uint64_t> d_carry;    // two carry lists and the drain's sorted list, (window + kCarryLanes) slots each
+	abb::DevBuf<unsigned> d_slotbits; // presence bitmap of the drain
 	uint64_t slotbit_words = 0;
-	unsigned* d_ctl = nullptr;             // abb::InsertCtl
-	unsigned long long* d_stats = nullptr; // [0] deferred [1] drains [2] slots replayed by drains [3..4] popcount scratch
+	abb::DevBuf<unsigned> d_ctl;             // abb::InsertCtl
+	abb::DevBuf<unsigned long long> d_stats; // [0] deferred [1] drains [2] slots replayed by drains [3..4] popcount scratch
 
 	// per-call buffers (bases/offs keep the device copy of the last host batch: abb_filter_resident_reads)
 	uint64_t resident_reads = 0;
@@ -157,6 +210,6 @@ struct abb_filter {
 	abb_insert_stats st = {};
 	bool profile = false; // time the k_window launches with CUDA events (every prof_stride-th window)
 	uint64_t prof_stride = 1, prof_slots = 0, sh_drains = 0;
-	std::vector<cudaEvent_t> prof_ev;
+	std::vector<abb::Event> prof_ev;
 	size_t prof_used = 0;
 };

@@ -10,7 +10,7 @@ using namespace abb;
 static KonView kon_view(const abb_filter* f)
 {
 	KonView v;
-	v.data = f->d_data;
+	v.data = f->d_data.p;
 	v.bytes_per_level = f->bytes_per_level;
 	v.bits = f->size;
 	v.start = f->kon_start;
@@ -38,7 +38,7 @@ int kon_insert_reads_dev(abb_filter* f, const uint8_t* d_bases, const uint64_t* 
 	ABB_CHECK(compute_slot_offsets(f->k, d_offs, n_reads, f->slot_offs, f->scan_tmp, f->stream, &total, &f->st.launches));
 	if (total == 0)
 		return ABB_OK;
-	unsigned long long* d_count = f->d_stats + 6;
+	unsigned long long* d_count = f->d_stats.p + 6;
 	ABB_CUDA(cudaMemsetAsync(d_count, 0, sizeof(unsigned long long), f->stream));
 	ABB_CUDA(cudaEventRecord(f->ev0, f->stream));
 	k_kon_walk<false><<<kon_grid(total), 256, 0, f->stream>>>(d_bases, d_offs, f->slot_offs.p, n_reads, total, kon_geom(f->k), kon_view(f),
@@ -93,7 +93,7 @@ int abb_filter_read_bits(abb_filter* f, int level, const uint8_t* host, uint64_t
 	ABB_CUDA(cudaMemcpyAsync(src.p, host, nbytes, cudaMemcpyHostToDevice, f->stream));
 	const uint64_t dest_bytes = bit_offset / 8 + nbytes + 1;
 	k_kon_read_bits<<<std::min<unsigned>(blocks_for(dest_bytes, 256), sm_count() * 16), 256, 0, f->stream>>>(
-	    f->d_data + (uint64_t)level * f->bytes_per_level, f->bytes_per_level, src.p, bits, bit_offset, op);
+	    f->d_data.p + (uint64_t)level * f->bytes_per_level, f->bytes_per_level, src.p, bits, bit_offset, op);
 	f->st.launches += 1;
 	ABB_CUDA(cudaGetLastError());
 	ABB_CUDA(cudaStreamSynchronize(f->stream));
@@ -108,9 +108,9 @@ int abb_filter_level_popcount(abb_filter* f, int level, uint64_t* n)
 		level = (int)f->levels - 1;
 	ABB_REQUIRE((unsigned)level < f->levels, "level %d out of range", level);
 	ABB_CUDA(cudaSetDevice(f->device));
-	unsigned long long* d_n = f->d_stats + 6;
+	unsigned long long* d_n = f->d_stats.p + 6;
 	ABB_CUDA(cudaMemsetAsync(d_n, 0, sizeof(unsigned long long), f->stream));
-	k_kon_popcount<<<sm_count() * 8, 256, 0, f->stream>>>(f->d_data + (uint64_t)level * f->bytes_per_level, f->bytes_per_level, d_n);
+	k_kon_popcount<<<sm_count() * 8, 256, 0, f->stream>>>(f->d_data.p + (uint64_t)level * f->bytes_per_level, f->bytes_per_level, d_n);
 	f->st.launches += 1;
 	ABB_CUDA(cudaGetLastError());
 	unsigned long long h = 0;
@@ -130,11 +130,11 @@ int abb_filter_compare(abb_filter* a, abb_filter* b, uint64_t counts[4])
 	ABB_REQUIRE(a->device == b->device, "the two filters are on different devices");
 	ABB_CUDA(cudaSetDevice(a->device));
 	ABB_CUDA(cudaStreamSynchronize(b->stream));
-	unsigned long long* d_c = a->d_stats + 5; // [5..7]
+	unsigned long long* d_c = a->d_stats.p + 5; // [5..7]
 	ABB_CUDA(cudaMemsetAsync(d_c, 0, 3 * sizeof(unsigned long long), a->stream));
 	const uint64_t nbytes = a->bytes_per_level;
 	k_kon_compare<<<std::min<unsigned>(blocks_for(nbytes, 256), sm_count() * 8), 256, 0, a->stream>>>(
-	    a->d_data + (uint64_t)(a->levels - 1) * nbytes, b->d_data + (uint64_t)(b->levels - 1) * nbytes, nbytes, d_c);
+	    a->d_data.p + (uint64_t)(a->levels - 1) * nbytes, b->d_data.p + (uint64_t)(b->levels - 1) * nbytes, nbytes, d_c);
 	a->st.launches += 1;
 	ABB_CUDA(cudaGetLastError());
 	unsigned long long h[3] = { 0, 0, 0 };

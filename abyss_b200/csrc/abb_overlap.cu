@@ -88,14 +88,14 @@ using namespace abb;
 
 struct abb_overlap {
 	int device = 0;
-	cudaStream_t stream = nullptr;
+	Stream stream;
 	DevBuf<uint8_t> bases, tmp;
 	DevBuf<uint64_t> offs, key_p, key_p2, key_s, cnt, pos, sub_key, sub_key2, sub_val, sub_val2, ekey, ekey2;
 	DevBuf<uint32_t> val_p, val_p2, blunt;
 	DevBuf<int> edist, edist2;
 	DevBuf<abb_overlap_edge> d_edges;
 	std::vector<abb_overlap_edge> edges;
-	unsigned* d_bad = nullptr;
+	DevBuf<unsigned> d_bad;
 	abb_overlap_stats st = {};
 };
 
@@ -140,11 +140,11 @@ static int overlap_build(abb_overlap* h, const char* bases, const uint64_t* offs
 	ABB_CHECK(h->offs.reserve(n + 1));
 	ABB_CUDA(cudaMemcpyAsync(h->bases.p, bases, n_bases, cudaMemcpyHostToDevice, st));
 	ABB_CUDA(cudaMemcpyAsync(h->offs.p, offsets, (n + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
-	ABB_CUDA(cudaMemsetAsync(h->d_bad, 0, 2 * sizeof(unsigned), st));
+	ABB_CUDA(cudaMemsetAsync(h->d_bad.p, 0, 2 * sizeof(unsigned), st));
 	OvlSeqs s = { h->bases.p, h->offs.p, n, k1 };
-	k_ovl_check_len<<<ovl_grid(n), 256, 0, st>>>(s, h->d_bad);
+	k_ovl_check_len<<<ovl_grid(n), 256, 0, st>>>(s, h->d_bad.p);
 	unsigned bad[2] = { 0, 0 };
-	ABB_CUDA(cudaMemcpyAsync(bad, h->d_bad, sizeof bad, cudaMemcpyDeviceToHost, st));
+	ABB_CUDA(cudaMemcpyAsync(bad, h->d_bad.p, sizeof bad, cudaMemcpyDeviceToHost, st));
 	ABB_CUDA(cudaStreamSynchronize(st));
 	ABB_REQUIRE(!bad[1], "a contig is not longer than k-1 = %u bases (AdjList asserts seq.length() > overlap)", k1);
 	// join (1): exact k-1 overlaps
@@ -154,14 +154,14 @@ static int overlap_build(abb_overlap* h, const char* bases, const uint64_t* offs
 	ABB_CHECK(h->val_p2.reserve(n2));
 	ABB_CHECK(h->key_s.reserve(n2));
 	ABB_CHECK(h->cnt.reserve(n2 + 1));
-	k_ovl_keys<<<ovl_grid(n2), 256, 0, st>>>(s, h->key_p.p, h->val_p.p, h->key_s.p, h->d_bad);
+	k_ovl_keys<<<ovl_grid(n2), 256, 0, st>>>(s, h->key_p.p, h->val_p.p, h->key_s.p, h->d_bad.p);
 	ABB_CUDA(cudaGetLastError());
 	ABB_CHECK(ovl_sort(h, h->key_p.p, h->key_p2.p, h->val_p.p, h->val_p2.p, n2)); // stable: equal keys stay in ascending t ^ 1
 	k_ovl_join<false><<<ovl_grid(n2), 256, 0, st>>>(s, ss, h->key_s.p, h->key_p2.p, h->val_p2.p, h->cnt.p, nullptr, nullptr);
 	ABB_CUDA(cudaGetLastError());
 	uint64_t e1 = 0;
 	ABB_CHECK(ovl_scan(h, h->cnt.p, n2, &e1));
-	ABB_CUDA(cudaMemcpyAsync(bad, h->d_bad, sizeof bad, cudaMemcpyDeviceToHost, st));
+	ABB_CUDA(cudaMemcpyAsync(bad, h->d_bad.p, sizeof bad, cudaMemcpyDeviceToHost, st));
 	ABB_CUDA(cudaStreamSynchronize(st));
 	ABB_REQUIRE(!bad[0], "a contig end holds a character that is not a nucleotide (the reference's Kmer constructor aborts on it)");
 	h->st.launches += 5;
@@ -206,10 +206,8 @@ static int overlap_build(abb_overlap* h, const char* bases, const uint64_t* offs
 			ABB_CUDA(cudaMemcpyAsync(nk.p, h->ekey.p, e1 * sizeof(uint64_t), cudaMemcpyDeviceToDevice, st));
 			ABB_CUDA(cudaMemcpyAsync(nd.p, h->edist.p, e1 * sizeof(int), cudaMemcpyDeviceToDevice, st));
 			ABB_CUDA(cudaStreamSynchronize(st));
-			h->ekey.release();
-			h->edist.release();
-			h->ekey = nk;
-			h->edist = nd;
+			h->ekey = std::move(nk);
+			h->edist = std::move(nd);
 			k_ovl_sub_join<true><<<ovl_grid(n_blunt), 256, 0, st>>>(s, ss, h->blunt.p, n_blunt, n_q, h->sub_key2.p, h->sub_val2.p, h->pos.p, h->ekey.p + e1,
 			                                                       h->edist.p + e1);
 			ABB_CUDA(cudaGetLastError());
@@ -245,22 +243,15 @@ int abb_overlap_create(abb_overlap** out, int device)
 	ABB_REQUIRE(out != nullptr, "abb_overlap_create: out is NULL");
 	*out = nullptr;
 	ABB_CHECK(select_device(device));
-	abb_overlap* h = new (std::nothrow) abb_overlap();
+	std::unique_ptr<abb_overlap> h(new (std::nothrow) abb_overlap());
 	if (!h) {
 		set_error("out of host memory");
 		return ABB_ENOMEM;
 	}
 	h->device = device;
-	cudaError_t e = cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking);
-	if (e == cudaSuccess)
-		e = cudaMalloc((void**)&h->d_bad, 2 * sizeof(unsigned));
-	if (e != cudaSuccess) {
-		set_error("abb_overlap_create: %s", cudaGetErrorString(e));
-		abb_overlap_destroy(h);
-		return ABB_ECUDA;
-	}
-	*out = h;
-	return ABB_OK;
+	ABB_CUDA(cudaStreamCreateWithFlags(h->stream.out(), cudaStreamNonBlocking));
+	ABB_CHECK(h->d_bad.alloc(2));
+	return hand_over(h, out);
 }
 
 int abb_overlap_destroy(abb_overlap* h)
@@ -268,15 +259,7 @@ int abb_overlap_destroy(abb_overlap* h)
 	if (!h)
 		return ABB_OK;
 	cudaSetDevice(h->device);
-	if (h->stream)
-		cudaStreamSynchronize(h->stream);
-	h->bases.release(); h->tmp.release(); h->offs.release(); h->key_p.release(); h->key_p2.release(); h->key_s.release();
-	h->cnt.release(); h->pos.release(); h->sub_key.release(); h->sub_key2.release(); h->sub_val.release(); h->sub_val2.release();
-	h->ekey.release(); h->ekey2.release(); h->val_p.release(); h->val_p2.release(); h->blunt.release(); h->edist.release();
-	h->edist2.release(); h->d_edges.release();
-	cudaFree(h->d_bad);
-	if (h->stream)
-		cudaStreamDestroy(h->stream);
+	cudaStreamSynchronize(h->stream);
 	delete h;
 	return ABB_OK;
 }

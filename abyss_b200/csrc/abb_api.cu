@@ -50,15 +50,6 @@ int select_device(int device)
 		return ABB_EINVAL;
 	}
 	ABB_CUDA(cudaSetDevice(device));
-	// tuning knob: ABB_L2_FETCH=32 asks L2 to fetch 32 B sectors from HBM (cudaLimitMaxL2FetchGranularity).
-	// Off by default: the Bloom accesses are random single bytes, and the hardware's default fetch size is kept.
-	static int fetch = -1;
-	if (fetch < 0) {
-		const char* e = getenv("ABB_L2_FETCH");
-		fetch = e ? atoi(e) : 0;
-	}
-	if (fetch > 0)
-		cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, (size_t)fetch);
 	return ABB_OK;
 }
 
@@ -74,17 +65,16 @@ static FilterView view_of(const abb_filter* f)
 /** conflict-map size: 2^25 two-bit entries (8 MiB per map; the three rotating maps are pinned in L2 while the insert
  *  runs, set_l2_policy); with the default window of 2^17 slots 6.4 % of the slots see an alias and are carried (2^26
  *  halves that and measured 3 % slower: the maps compete with the counter sectors for L2).  Exact (no aliases) for
- *  filters of up to 2^25 positions.  ABB_MAP_LOG2 overrides (tuning). */
-static uint64_t map_entries_for(uint64_t filter_size, unsigned lg = 25)
+ *  filters of up to 2^25 positions. */
+constexpr unsigned kMapLog2 = 25;
+/** the sharded insert's maps: each rank marks window * H / world positions, 2^20 at the default window */
+constexpr unsigned kShardMapLog2 = 27;
+
+/** entries per conflict map: 2^lg, or fewer when the filter has fewer positions */
+static uint64_t map_entries_for(uint64_t filter_size, unsigned lg)
 {
-	if (const char* e = getenv("ABB_MAP_LOG2")) {
-		const int v = atoi(e);
-		if (v >= 10 && v <= 32)
-			lg = (unsigned)v;
-	}
-	uint64_t want = 1ULL << lg;
 	const uint64_t fit = std::max<uint64_t>(next_pow2(filter_size), 1024);
-	return std::min(want, fit);
+	return std::min<uint64_t>(1ULL << lg, fit);
 }
 
 static unsigned age_windows_for(uint64_t window)
@@ -92,11 +82,12 @@ static unsigned age_windows_for(uint64_t window)
 	return (unsigned)std::min<uint64_t>(kMaxAgeWindows, ((1ULL << kPrioBits) - 2) / window - 1);
 }
 
-/** make sure the ordered-insert workspace exists for the current window size and hash count */
-static int ensure_workspace(abb_filter* f)
+/** make sure the ordered-insert workspace exists for `window` slots per window, conflict maps of 2^lg entries (at
+ *  most) and the current hash count */
+static int ensure_workspace(abb_filter* f, uint64_t window, unsigned lg)
 {
-	const uint64_t want_entries = map_entries_for(f->size, f->map_log2 ? f->map_log2 : 25);
-	if (f->d_carry.p && f->ws_window == f->window && f->ws_H == f->H && f->map_entries == want_entries)
+	const uint64_t want_entries = map_entries_for(f->size, lg);
+	if (f->d_carry.p && f->ws_window == window && f->ws_H == f->H && f->map_entries == want_entries)
 		return ABB_OK;
 	// the old workspace is freed before the new one is allocated (peak memory), and it counts as valid again only once
 	// every piece has been allocated
@@ -118,15 +109,15 @@ static int ensure_workspace(abb_filter* f)
 		ABB_CUDA(cudaMemsetAsync(tags.p, 0, f->tag_slots * sizeof(unsigned long long), f->stream));
 	}
 	// worst case everything defers: window slots + the carried lanes, twice, plus the drain's sorted copy
-	ABB_CHECK(f->d_carry.alloc(3 * (f->window + kCarryLanes)));
+	ABB_CHECK(f->d_carry.alloc(3 * (window + kCarryLanes)));
 	// presence bitmap of the drain: pending slots span at most age_off + 2 windows
-	f->slotbit_words = ((uint64_t)age_windows_for(f->window) + 3) * f->window / 32 + 64;
+	f->slotbit_words = ((uint64_t)age_windows_for(window) + 3) * window / 32 + 64;
 	ABB_CHECK(f->d_slotbits.alloc(f->slotbit_words));
 	ABB_CUDA(cudaMemsetAsync(f->d_slotbits.p, 0, f->slotbit_words * sizeof(unsigned), f->stream));
 	for (int i = 0; i < 3; ++i)
 		f->d_map[i] = f->maps.p + i * map_words;
 	f->map_entries = want_entries;
-	f->ws_window = f->window;
+	f->ws_window = window;
 	f->ws_H = f->H;
 	return ABB_OK;
 }
@@ -148,16 +139,9 @@ static int ensure_workspace(abb_filter* f)
 /** While the insert runs, the two conflict maps are pinned in L2 (persisting access-policy window on the filter's stream)
  *  and everything else -- the random counter sectors, the hashes -- is treated as streaming, so that 30-60 MB of counter
  *  lines per window cannot push the maps out (ncu, round 2: without this 57 % of the map atomics missed L2 and the kernel
- *  moved 3x the algorithmic DRAM bytes).  ABB_L2_PERSIST=0 switches it off (tuning). */
+ *  moved 3x the algorithmic DRAM bytes). */
 static void set_l2_policy(abb_filter* f, bool on, int n_maps = 3)
 {
-	static int enabled = -1;
-	if (enabled < 0) {
-		const char* e = getenv("ABB_L2_PERSIST");
-		enabled = e ? atoi(e) : 1;
-	}
-	if (!enabled)
-		return;
 	cudaStreamAttrValue attr;
 	memset(&attr, 0, sizeof attr);
 	if (on) {
@@ -227,6 +211,24 @@ static int launch_windows(const InsertArgs& args, int device, cudaStream_t st)
 	return ABB_OK;
 }
 
+/** fold the timed insert launches (event pairs in f->prof_ev) of one call into the statistics */
+static int fold_profile(abb_filter* f)
+{
+	if (!f->profile || !f->prof_used)
+		return ABB_OK;
+	ABB_CUDA(cudaStreamSynchronize(f->stream));
+	for (size_t i = 0; i + 1 < f->prof_used; i += 2) {
+		float ms = 0;
+		cudaEventElapsedTime(&ms, f->prof_ev[i], f->prof_ev[i + 1]);
+		f->st.ms_commit += ms;
+		f->st.commit_launches += 1;
+	}
+	f->st.commit_slots += f->prof_slots;
+	f->prof_used = 0;
+	f->prof_slots = 0;
+	return ABB_OK;
+}
+
 /** ordered insert of slots [0, n_slots) of `hashes` (h0 per slot, or literal H per slot); see abb_insert.cuh */
 template <bool LITERAL>
 static int ordered_insert(abb_filter* f, const uint64_t* d_hashes, const uint8_t* d_valid, uint64_t n_slots)
@@ -240,7 +242,7 @@ static int ordered_insert(abb_filter* f, const uint64_t* d_hashes, const uint8_t
 		ABB_CUDA(cudaGetLastError());
 		return ABB_OK;
 	}
-	ABB_CHECK(ensure_workspace(f));
+	ABB_CHECK(ensure_workspace(f, f->window, kMapLog2));
 	cudaStream_t st = f->stream;
 	const uint64_t W = f->window;
 	const uint64_t n_windows = (n_slots + W - 1) / W;
@@ -268,7 +270,6 @@ static int ordered_insert(abb_filter* f, const uint64_t* d_hashes, const uint8_t
 	a.drain_age = a.age_off / 3 * 2;
 	a.ctl = reinterpret_cast<InsertCtl*>(f->d_ctl.p);
 	a.stats = f->d_stats.p;
-	a.dbg = getenv("ABB_DBG") ? (unsigned)atoi(getenv("ABB_DBG")) : 0u;
 	uint64_t* sorted = f->d_carry.p + 2 * cap;
 	// the maps, both tag tables and the control block start clean
 	ABB_CUDA(cudaMemsetAsync(f->d_ctl.p, 0, sizeof(InsertCtl), st));
@@ -312,19 +313,7 @@ static int ordered_insert(abb_filter* f, const uint64_t* d_hashes, const uint8_t
 		a.w_begin = h.resume;
 	}
 	ABB_CUDA(cudaGetLastError());
-	if (f->profile && f->prof_used) { // fold the timed k_insert_windows launches into the statistics
-		ABB_CUDA(cudaStreamSynchronize(st));
-		for (size_t i = 0; i + 1 < f->prof_used; i += 2) {
-			float ms = 0;
-			cudaEventElapsedTime(&ms, f->prof_ev[i], f->prof_ev[i + 1]);
-			f->st.ms_commit += ms;
-			f->st.commit_launches += 1;
-		}
-		f->st.commit_slots += f->prof_slots;
-		f->prof_used = 0;
-		f->prof_slots = 0;
-	}
-	return ABB_OK;
+	return fold_profile(f);
 }
 
 /** single thread: cut reads into chunks of about `cap` slots (at least one read per chunk) */
@@ -367,39 +356,34 @@ k_count_valid(const uint8_t* __restrict__ valid, uint64_t n, unsigned long long*
 }
 
 /** K1 launcher for reads [r0, r1): h0/valid index = slot_offs[r] + j - slot_base */
-int launch_hash(abb_filter* f, unsigned k, const uint8_t* d_care, const uint8_t* d_bases,
-                       const uint64_t* d_offs, const uint64_t* d_slot_offs, uint64_t r0, uint64_t r1,
-                       uint64_t slot_base, uint64_t* d_h0, uint8_t* d_valid, cudaStream_t stream, uint64_t* launches)
+int launch_hash(unsigned k, const uint8_t* d_care, const uint8_t* d_bases, const uint64_t* d_offs, const uint64_t* d_slot_offs,
+                uint64_t r0, uint64_t r1, uint64_t slot_base, uint64_t* d_h0, uint8_t* d_valid, cudaStream_t stream, uint64_t* launches)
 {
-	(void)f;
 	const uint64_t n = r1 - r0;
 	if (n == 0)
 		return ABB_OK;
-	int sms = 132, dev = 0;
-	cudaGetDevice(&dev);
-	cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-	const unsigned grid = (unsigned)std::min<uint64_t>((n + kHashWarps - 1) / kHashWarps, (uint64_t)sms * 32);
-	// ABB_TMA=0: K1 without the bulk-copy staging (tuning / fallback).  The opt-in to 56 KB of shared memory is a per-device
-	// attribute of the kernel: a process that drives several GPUs (abyss-bloom-dbg --devices) sets it on each of them.
-	static int tma_env = -1;
-	static int tma_dev[64] = { 0 }; // 0 = not tried on this device, 1 = usable, -1 = not usable
-	if (tma_env < 0) {
-		const char* e = getenv("ABB_TMA");
-		tma_env = e ? atoi(e) : 1;
-	}
-	int& tma_here = tma_dev[dev & 63];
-	if (tma_env && tma_here == 0)
-		tma_here = cudaFuncSetAttribute(k_hash_reads_tma, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * kTmaStage) == cudaSuccess ? 1 : -1;
-	const bool tma = tma_env && tma_here == 1;
-	if (d_care)
+	const uint64_t sms = sm_count();
+	if (d_care) {
+		const unsigned grid = (unsigned)std::min<uint64_t>((n + kHashWarps - 1) / kHashWarps, sms * 32);
 		k_hash_reads_masked<<<grid, kHashWarps * 32, 0, stream>>>(d_bases, d_offs + r0, d_slot_offs + r0, slot_base, n, k, d_care,
 		                                                          d_h0, d_valid);
-	else if (tma && (reinterpret_cast<uintptr_t>(d_bases) & 15) == 0) {
-		// read blocks staged into shared memory by the bulk-copy engine (cp.async.bulk), double buffered
-		const unsigned g = (unsigned)std::min<uint64_t>((n + kTmaReads - 1) / kTmaReads, (uint64_t)sms * 4);
-		k_hash_reads_tma<<<g, kHashWarps * 32, 2 * kTmaStage, stream>>>(d_bases, d_offs + r0, d_slot_offs + r0, slot_base, n, k, d_h0, d_valid);
-	} else
-		k_hash_reads<<<grid, kHashWarps * 32, 0, stream>>>(d_bases, d_offs + r0, d_slot_offs + r0, slot_base, n, k, d_h0, d_valid);
+	} else {
+		// The opt-in to 16 KB of dynamic shared memory (56 KB in all) is a per-device attribute of the kernel: a process that
+		// drives several GPUs (abyss-bloom-dbg --devices) sets it on each of them.
+		static bool smem_opt_in[64] = {};
+		int dev = 0;
+		ABB_CUDA(cudaGetDevice(&dev));
+		if (!smem_opt_in[dev & 63]) {
+			ABB_CUDA(cudaFuncSetAttribute(k_hash_reads_tma, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * kTmaStage));
+			smem_opt_in[dev & 63] = true;
+		}
+		// read blocks staged into shared memory by the bulk-copy engine (cp.async.bulk), double buffered; the copy needs a
+		// 16-byte aligned source, so reads at an unaligned base pointer are all hashed from global memory
+		const bool may_stage = (reinterpret_cast<uintptr_t>(d_bases) & 15) == 0;
+		const unsigned grid = (unsigned)std::min<uint64_t>((n + kTmaReads - 1) / kTmaReads, sms * 4);
+		k_hash_reads_tma<<<grid, kHashWarps * 32, 2 * kTmaStage, stream>>>(d_bases, d_offs + r0, d_slot_offs + r0, slot_base, n, k,
+		                                                                  d_h0, d_valid, may_stage);
+	}
 	if (launches)
 		*launches += 1;
 	ABB_CUDA(cudaGetLastError());
@@ -517,8 +501,8 @@ static int insert_reads_dev(abb_filter* f, const uint8_t* d_bases, const uint64_
 		if (pc)
 			ABB_CHECK(wait_bases(f, pc, pc->h_offs[r1]));
 		ABB_CUDA(cudaEventRecord(f->ev0, f->stream));
-		ABB_CHECK(launch_hash(f, f->k, f->d_care.p, d_bases, d_offs, f->slot_offs.p, r0, r1, slot_at[c], f->h0.p, f->valid.p,
-		                      f->stream, &f->st.launches));
+		ABB_CHECK(launch_hash(f->k, f->d_care.p, d_bases, d_offs, f->slot_offs.p, r0, r1, slot_at[c], f->h0.p, f->valid.p, f->stream,
+		                      &f->st.launches));
 		k_count_valid<<<std::min<unsigned>(blocks_for(slots, 256), sm_count() * 8), 256, 0, f->stream>>>(f->valid.p, slots, f->d_stats.p + 3);
 		f->st.launches += 1;
 		ABB_CUDA(cudaEventRecord(f->ev1, f->stream));
@@ -623,9 +607,7 @@ static uint64_t shard_chunk(uint64_t size, unsigned world) { return ((size + wor
 /** the window of the sharded pipeline: per-rank conflict-map load like the single-GPU window */
 static uint64_t sharded_window(const abb_filter* f, unsigned world)
 {
-	uint64_t w = 2 * f->window * world; // 2^18 slots per rank: the per-rank conflict-map load of the single-GPU window, twice
-	if (const char* e = getenv("ABB_SHARD_WINDOW"))
-		w = strtoull(e, nullptr, 10);
+	const uint64_t w = 2 * f->window * world; // 2^18 slots per rank: the per-rank conflict-map load of the single-GPU window, twice
 	return std::min<uint64_t>(std::max<uint64_t>(w, 32), 1ULL << 21);
 }
 
@@ -633,14 +615,8 @@ static int sharded_ordered_insert(abb_filter* f, abb_comm* c, const uint64_t* d_
 {
 	if (n_slots == 0)
 		return ABB_OK;
-	const uint64_t user_window = f->window;
-	f->window = sharded_window(f, (unsigned)c->world);
-	f->map_log2 = 27; // each rank marks window * H / world positions: 2^20 at the default window
-	int rc = ensure_workspace(f);
-	const uint64_t W = f->window;
-	f->window = user_window;
-	f->map_log2 = 0;
-	ABB_CHECK(rc);
+	const uint64_t W = sharded_window(f, (unsigned)c->world);
+	ABB_CHECK(ensure_workspace(f, W, kShardMapLog2));
 	// carried slots served per step: the tag table holds only own positions, so world times the single-GPU number fit
 	const unsigned max_lanes = (unsigned)std::min<uint64_t>((uint64_t)kCarryLanes * (unsigned)c->world, W / 2 + kCarryLanes);
 	ABB_CHECK(f->sh_buf.reserve(2 * (W + (uint64_t)max_lanes) + 64));
@@ -706,8 +682,8 @@ static int sharded_ordered_insert(abb_filter* f, abb_comm* c, const uint64_t* d_
 			k_sh_compact<<<1, kDrainThreads, 0, st>>>(f->d_slotbits.p, lo_slot, w0 + std::max<uint64_t>(n, 1), carry[1 - in], ctl, d_nout);
 			unsigned h_n = 0;
 			ABB_CUDA(cudaMemcpyAsync(&h_n, d_nout, sizeof h_n, cudaMemcpyDeviceToHost, st));
-			if (h_n || true) // the oldest pending slot bounds the priorities
-				ABB_CUDA(cudaMemcpyAsync(&oldest, carry[1 - in], sizeof oldest, cudaMemcpyDeviceToHost, st));
+			// the oldest pending slot bounds the priorities
+			ABB_CUDA(cudaMemcpyAsync(&oldest, carry[1 - in], sizeof oldest, cudaMemcpyDeviceToHost, st));
 			ABB_CUDA(cudaStreamSynchronize(st));
 			n_in = h_n;
 			in = 1 - in;
@@ -747,18 +723,7 @@ static int sharded_ordered_insert(abb_filter* f, abb_comm* c, const uint64_t* d_
 	}
 	ABB_CHECK(drain(n_slots, 0));
 	ABB_CUDA(cudaGetLastError());
-	if (f->profile && f->prof_used) {
-		ABB_CUDA(cudaStreamSynchronize(st));
-		for (size_t i = 0; i + 1 < f->prof_used; i += 2) {
-			float ms = 0;
-			cudaEventElapsedTime(&ms, f->prof_ev[i], f->prof_ev[i + 1]);
-			f->st.ms_commit += ms;
-			f->st.commit_launches += 1;
-		}
-		f->st.commit_slots += f->prof_slots;
-		f->prof_used = 0;
-		f->prof_slots = 0;
-	}
+	ABB_CHECK(fold_profile(f));
 	// leave the shared control block in the single-GPU layout
 	ABB_CUDA(cudaMemsetAsync(f->d_ctl.p, 0, 8 * sizeof(unsigned), st));
 	return ABB_OK;
@@ -990,21 +955,16 @@ int abb_insert_reads(abb_filter* f, const char* bases, const uint64_t* offsets, 
 	}
 	// The bases travel in pieces on a second stream; chunk c of the insert only waits for the pieces that hold its reads, so
 	// the copy of the rest hides behind the hashing and inserting of the earlier chunks (with pinned host memory; a pageable
-	// buffer makes cudaMemcpyAsync synchronous and the order is simply copy, then insert).  ABB_H2D_OVERLAP=0: one copy up front.
-	static int overlap = -1;
-	if (overlap < 0) {
-		const char* e = getenv("ABB_H2D_OVERLAP");
-		overlap = e ? atoi(e) : 1;
-	}
+	// buffer makes cudaMemcpyAsync synchronous and the order is simply copy, then insert).  One piece: one copy up front.
 	constexpr uint64_t kPiece = 256ULL << 20;
-	if (!overlap || n_bases <= kPiece) {
+	if (n_bases <= kPiece) {
 		ABB_CUDA(cudaMemcpyAsync(f->bases.p, bases, n_bases, cudaMemcpyHostToDevice, f->stream));
 		return insert_reads_dev(f, f->bases.p, f->offs.p, n_reads, n_kmers_out);
 	}
 	if (!f->copy_stream)
 		ABB_CUDA(cudaStreamCreateWithFlags(f->copy_stream.out(), cudaStreamNonBlocking));
 	if (f->kind != ABB_BIT)
-		ABB_CHECK(ensure_workspace(f)); // the maps exist before the policy that pins them is set
+		ABB_CHECK(ensure_workspace(f, f->window, kMapLog2)); // the maps exist before the policy that pins them is set
 	PolicyHold policy(f, 3); // before the copy starts: setting it later would wait for the whole copy (see PolicyHold)
 	PendingCopy pc;
 	pc.h_offs = offsets;
@@ -1127,7 +1087,7 @@ int abb_hash_reads_dev(abb_filter* f, const char* d_bases, const uint64_t* d_off
 	if (total == 0 || !d_h0 || !d_valid)
 		return ABB_OK;
 	ABB_REQUIRE(capacity >= total, "output buffers hold %llu slots, %llu needed", (unsigned long long)capacity, (unsigned long long)total);
-	ABB_CHECK(launch_hash(f, f->k, f->d_care.p, (const uint8_t*)d_bases, d_offsets, f->slot_offs.p, 0, n_reads, 0, d_h0, d_valid, f->stream,
+	ABB_CHECK(launch_hash(f->k, f->d_care.p, (const uint8_t*)d_bases, d_offsets, f->slot_offs.p, 0, n_reads, 0, d_h0, d_valid, f->stream,
 	                      &f->st.launches));
 	ABB_CUDA(cudaStreamSynchronize(f->stream));
 	return ABB_OK;
@@ -1337,7 +1297,7 @@ int abb_contains_reads(abb_filter* f, const char* bases, const uint64_t* offsets
 		ABB_CHECK(kon_query_slots(f, d_bases.p, d_offs.p, n_reads, total));
 	else {
 		ABB_CHECK(f->h0.reserve(total));
-		ABB_CHECK(launch_hash(f, f->k, f->d_care.p, d_bases.p, d_offs.p, f->slot_offs.p, 0, n_reads, 0, f->h0.p, f->valid.p, f->stream, &f->st.launches));
+		ABB_CHECK(launch_hash(f->k, f->d_care.p, d_bases.p, d_offs.p, f->slot_offs.p, 0, n_reads, 0, f->h0.p, f->valid.p, f->stream, &f->st.launches));
 		const FilterView fv = view_of(f);
 		const unsigned grid = std::min<unsigned>(blocks_for(total, 256), sm_count() * 16);
 		if (f->kind == ABB_COUNTING)
@@ -1431,8 +1391,8 @@ int abb_hash_reads(unsigned k, const char* mask, const char* bases, const uint64
 	if (total && out_h0 && out_valid) {
 		ABB_CHECK(d_h0.reserve(total));
 		ABB_CHECK(d_valid.reserve(total));
-		ABB_CHECK(launch_hash(nullptr, k, m.empty() ? nullptr : d_care.p, d_bases.p, d_offs.p, d_slot.p, 0, n_reads, 0, d_h0.p,
-		                      d_valid.p, 0, nullptr));
+		ABB_CHECK(launch_hash(k, m.empty() ? nullptr : d_care.p, d_bases.p, d_offs.p, d_slot.p, 0, n_reads, 0, d_h0.p, d_valid.p, 0,
+		                      nullptr));
 		ABB_CUDA(cudaMemcpy(out_h0, d_h0.p, total * sizeof(uint64_t), cudaMemcpyDeviceToHost));
 		ABB_CUDA(cudaMemcpy(out_valid, d_valid.p, total, cudaMemcpyDeviceToHost));
 	}

@@ -62,18 +62,6 @@ struct WarpCtx {
 	const unsigned* tile_tab; // open addressing: tile index + 1, 0 = empty
 	unsigned tile_mask;
 
-	// profiling hook (ABB_ROUND_LOG): clock64 ticks between the stages of a walk, accumulated per speculated read
-	unsigned long long* dbg = nullptr;
-	long long t_last = 0;
-	__device__ void tick(int slot)
-	{
-		if (!dbg)
-			return;
-		const long long now = clock64();
-		if (slot >= 0 && lane == 0)
-			dbg[slot] += (unsigned long long)(now - t_last);
-		t_last = now;
-	}
 	__device__ bool tiles_enabled() const { return tile_tab != nullptr; }
 	__device__ const TileRec* tile_lookup(uint64_t key, unsigned cls) const
 	{
@@ -586,13 +574,12 @@ __global__ void __launch_bounds__(kWalkWarps * 32)
 k_extend(const uint8_t* __restrict__ bases, const uint64_t* __restrict__ offs, const unsigned* __restrict__ spec, unsigned n_spec,
          WalkCfg w, const __grid_constant__ HashCfg cfg, Frame* frames, uint64_t* look, uint8_t* arena,
          unsigned long long arena_size, unsigned long long* arena_top, ContigRec* recs, unsigned* nrecs, unsigned rec_cap,
-         unsigned* __restrict__ status, TileView tv, unsigned long long* dbg)
+         unsigned* __restrict__ status, TileView tv)
 {
 	const unsigned gwarp = blockIdx.x * kWalkWarps + (threadIdx.x >> 5);
 	if (gwarp >= n_spec)
 		return;
 	WarpCtx c = make_ctx(w, &cfg, frames, look, gwarp, arena, arena_size, arena_top);
-	c.dbg = dbg ? dbg + 4ull * gwarp : nullptr;
 	c.tile_recs = tv.recs;
 	c.tile_tab = tv.tab;
 	c.tile_mask = tv.mask;
@@ -1234,7 +1221,7 @@ struct abb_assembler {
 	DevBuf<unsigned long long> d_tile_pool_top;
 	DevBuf<unsigned long long> d_marker_set;
 	unsigned marker_set_mask = 0;
-	DevBuf<unsigned long long> new_markers, rep_tab, walk_dbg;
+	DevBuf<unsigned long long> new_markers, rep_tab;
 	DevBuf<TileRec> tile_export;
 	DevBuf<uint8_t> stage_bases, rep_flag;
 	DevBuf<uint64_t> stage_hashes;
@@ -1243,7 +1230,6 @@ struct abb_assembler {
 
 	// speculation control
 	unsigned spec_target = 512;
-	unsigned spec_fixed = 0;
 	// host outputs of the last batch
 	std::vector<abb_contig> out_contigs;
 	std::vector<char> out_seqs;
@@ -1574,12 +1560,6 @@ int run_extend(abb_assembler* a, unsigned n_spec, bool use_tiles, bool keep_aren
 	}
 	for (;;) {
 		ABB_CHECK(a->recs.reserve(rec_cap));
-		unsigned long long* dbg = nullptr;
-		if (getenv("ABB_ROUND_LOG")) {
-			ABB_CHECK(a->walk_dbg.reserve(4ull * n_spec));
-			ABB_CUDA(cudaMemsetAsync(a->walk_dbg.p, 0, 4ull * n_spec * sizeof(unsigned long long), st));
-			dbg = a->walk_dbg.p;
-		}
 		ABB_CHECK(ensure_arena(a, a->arena_size ? a->arena_size : std::max(kArenaDefault, g_arena_hint)));
 		ABB_CUDA(cudaMemcpyAsync(a->d_arena_top.p, &arena_mark, sizeof arena_mark, cudaMemcpyHostToDevice, st));
 		ABB_CUDA(cudaMemsetAsync(a->d_nrecs.p, 0, sizeof(unsigned), st));
@@ -1588,7 +1568,7 @@ int run_extend(abb_assembler* a, unsigned n_spec, bool use_tiles, bool keep_aren
 		cudaEventRecord(a->ev2[0], st);
 		ABB_DISPATCH_KW(a->kw, (k_extend<KW><<<blocks_for(n_spec, kWalkWarps), kWalkWarps * 32, 0, st>>>(
 		                           a->cur_bases, a->cur_offs, a->spec.p, n_spec, w, f->cfg, a->frames.p, a->look.p, a->d_arena.p, a->arena_size,
-		                           a->d_arena_top.p, a->recs.p, a->d_nrecs.p, rec_cap, a->status.p, tv, dbg)));
+		                           a->d_arena_top.p, a->recs.p, a->d_nrecs.p, rec_cap, a->status.p, tv)));
 		ABB_CUDA(cudaGetLastError());
 		cudaEventRecord(a->ev2[1], st);
 		++a->st_launches;
@@ -1600,21 +1580,6 @@ int run_extend(abb_assembler* a, unsigned n_spec, bool use_tiles, bool keep_aren
 			float ms = 0;
 			cudaEventElapsedTime(&ms, a->ev2[0], a->ev2[1]);
 			a->ms_walk += ms;
-		}
-		if (dbg) { // the slowest walk of this launch, by stage (SM clock ticks -> ms at 1.9 GHz)
-			std::vector<unsigned long long> h(4ull * n_spec);
-			cudaMemcpy(h.data(), dbg, h.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost);
-			unsigned best = 0;
-			unsigned long long bt = 0;
-			for (unsigned i = 0; i < n_spec; ++i) {
-				const unsigned long long t = h[4 * i] + h[4 * i + 1] + h[4 * i + 2] + h[4 * i + 3];
-				if (t > bt) {
-					bt = t;
-					best = i;
-				}
-			}
-			fprintf(stderr, "  k_extend %u walkers: slowest #%u extend-left %.1f extend-right %.1f materialise+trim %.1f mark_covered %.1f ms\n", n_spec, best,
-			        h[4 * best] / 1.9e6, h[4 * best + 1] / 1.9e6, h[4 * best + 2] / 1.9e6, h[4 * best + 3] / 1.9e6);
 		}
 		if (nrecs > rec_cap) { // record buffer too small: rerun with room for everything
 			rec_cap = nrecs + nrecs / 4 + 16;
@@ -1764,8 +1729,6 @@ int speculate_round(abb_assembler* a, const std::vector<unsigned>& cand, size_t*
 		return ABB_OK;
 	++a->st_iterations;
 	a->st_speculated += spec.size();
-	const float round_walk0 = a->ms_walk, round_rep0 = a->ms_repeat, round_vis0 = a->ms_visited, round_replay0 = a->ms_replay;
-	const auto round_t0 = std::chrono::steady_clock::now();
 
 	// ---- K4: extend all speculated reads (tiles on), then the exact vertex-by-vertex fallback for
 	// reads whose tiled walk cycled or produced a path with a repeated vertex
@@ -2009,19 +1972,8 @@ int speculate_round(abb_assembler* a, const std::vector<unsigned>& cand, size_t*
 		}
 	}
 	a->st_wasted += wasted;
-	if (getenv("ABB_ROUND_LOG")) { // tuning aid: one line per speculation round
-		unsigned long long longest = 0, accepted = 0;
-		for (unsigned c = 0; c < nc; ++c) {
-			longest = std::max<unsigned long long>(longest, clen[c]);
-			accepted += caccept[c] ? 1 : 0;
-		}
-		fprintf(stderr, "round %llu: speculated %u wasted %u contigs %u accepted %llu longest %llu | visited %.1f walk %.1f repeat %.1f replay %.1f ms, wall %.1f ms\n",
-		        (unsigned long long)a->st_iterations, n_ok, wasted, nc, accepted, longest, a->ms_visited - round_vis0, a->ms_walk - round_walk0,
-		        a->ms_repeat - round_rep0, a->ms_replay - round_replay0,
-		        std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - round_t0).count());
-	}
 	// adapt the amount of speculation: grow while most speculated reads were really needed
-	if (n_ok == n_spec && !a->spec_fixed) {
+	if (n_ok == n_spec) {
 		if (wasted * 2 <= n_ok)
 			a->spec_target = std::min(kMaxSpec, a->spec_target * 2);
 		else if (wasted * 20 > n_ok * 19)
@@ -2080,8 +2032,6 @@ int abb_assembler_create(abb_assembler** out, abb_filter* solid, const abb_assem
 	// tiles are keyed by vertex hash and assume that equal hashes continue identically; with a spaced seed two k-mers
 	// can share the hash and differ on the don't-care positions, so those runs walk vertex by vertex
 	a->tiles_on = getenv("ABB_NO_TILES") == nullptr && solid->mask.empty(); // env: debugging switch
-	if (const char* sp = getenv("ABB_SPEC")) // tuning switch: fixed speculation width
-		a->spec_fixed = a->spec_target = (unsigned)std::max(1, atoi(sp));
 	// BloomFilter assembledKmerSet(solid.size(), solid.getHashNum(), solid.getKmerSize()) (bloom-dbg.h:910-911)
 	abb_filter* assembled = nullptr;
 	ABB_CHECK(abb_filter_create(&assembled, ABB_BIT, solid->size, solid->H, solid->k, 0, "", solid->device));
@@ -2118,7 +2068,7 @@ static int hash_and_classify(abb_assembler* a, const uint8_t* d_bases, const uin
 	ABB_CHECK(a->valid.reserve(total + 1));
 	ABB_CHECK(a->codes.reserve(n_reads));
 	if (total)
-		ABB_CHECK(launch_hash(nullptr, f->k, f->d_care.p, d_bases, d_offs, a->slot_offs.p, 0, n_reads, 0, a->h0.p, a->valid.p, st,
+		ABB_CHECK(launch_hash(f->k, f->d_care.p, d_bases, d_offs, a->slot_offs.p, 0, n_reads, 0, a->h0.p, a->valid.p, st,
 		                      &a->st_launches));
 	*total_out = total;
 	if (!classify)
@@ -2321,7 +2271,7 @@ int abb_assembler_reset(abb_assembler* a)
 	ABB_CUDA(cudaStreamSynchronize(st));
 	a->counters = abb_assembly_counters{};
 	a->reads_seen = 0;
-	a->spec_target = a->spec_fixed ? a->spec_fixed : 512;
+	a->spec_target = 512;
 	a->st_iterations = a->st_speculated = a->st_wasted = a->st_launches = a->st_candidates = a->st_contigs_tried = 0;
 	a->st_markers = a->st_tiles = a->st_fallbacks = 0;
 	a->ms_classify = a->ms_visited = a->ms_extend = a->ms_replay = a->ms_tiles = a->ms_walk = a->ms_stage = a->ms_repeat = a->ms_total = a->ms_cand = 0;

@@ -148,9 +148,8 @@ int compute_slot_offsets(unsigned k, const uint64_t* d_offs, uint64_t n_reads, D
 struct abb_filter;
 namespace abb {
 /** K1 for reads [r0, r1): h0/valid index = slot_offs[r] + j - slot_base */
-int launch_hash(abb_filter* f, unsigned k, const uint8_t* d_care, const uint8_t* d_bases, const uint64_t* d_offs,
-                const uint64_t* d_slot_offs, uint64_t r0, uint64_t r1, uint64_t slot_base, uint64_t* d_h0, uint8_t* d_valid,
-                cudaStream_t stream, uint64_t* launches);
+int launch_hash(unsigned k, const uint8_t* d_care, const uint8_t* d_bases, const uint64_t* d_offs, const uint64_t* d_slot_offs,
+                uint64_t r0, uint64_t r1, uint64_t slot_base, uint64_t* d_h0, uint8_t* d_valid, cudaStream_t stream, uint64_t* launches);
 int launch_hash_segments(unsigned k, const uint8_t* d_care, const uint8_t* d_bases, const uint64_t* d_seg_beg, const unsigned* d_seg_len,
                          const uint64_t* d_seg_slot, uint64_t n_segs, uint64_t* d_h0, uint8_t* d_valid, cudaStream_t stream);
 // abb_konnector.cu: the ABB_KONNECTOR paths of abb_insert_reads(_dev) and abb_contains_reads
@@ -182,7 +181,6 @@ struct abb_filter {
 	uint64_t ws_window = 0;   // window the workspace below was sized for
 	unsigned ws_H = 0;
 	uint64_t map_entries = 0; // two-bit entries per conflict map (power of two)
-	unsigned map_log2 = 0;    // 0 = default size
 	abb::DevBuf<unsigned> maps;                         // the three maps in one allocation (one L2 access-policy window covers them)
 	unsigned* d_map[3] = { nullptr, nullptr, nullptr }; // the maps within `maps`
 	abb::DevBuf<unsigned long long> d_tags2[2];         // tag tables of the carried slots (alternating windows)

@@ -385,7 +385,7 @@ ABB_HD unsigned ctz4(unsigned m) { return (m & 1) ? 0 : (m & 2) ? 1 : (m & 4) ? 
  *   void copy8(dst, src, n), copy8_rev(dst, src, n)   cooperative byte copies (rev: dst[i] = src[n-1-i])
  *   void rehash(old, oldcap, new, newcap)              cooperative PathSet growth
  *   bool tiles_enabled(); const TileRec* tile_lookup(key, cls); const TileRec* tile_at(idx); void prefetch(const void*);
- *   uint32_t tile_index(const TileRec*); void wr32(uint32_t*, uint32_t); void tick(int) (profiling hook, may be empty)
+ *   uint32_t tile_index(const TileRec*); void wr32(uint32_t*, uint32_t)
  *   void mark_covered(ps, rh, cov, nk, contig)         cooperative: flag read k-mers that lie on the contig path
  *   Frame* frames; uint64_t* look;   per-warp scratch
  */
@@ -1029,13 +1029,10 @@ ABB_HD bool extend_seed(Ctx& c, const Vtx<KW>& seed, PathSet& ps, ContigOut* o)
 	o->pushed_front = o->pushed_back = false;
 	unsigned psize = 1;
 	Vtx<KW> front = seed, back = seed;
-	c.tick(-1);
 	o->left = extend_dir(c, front, REV, &psize, left, ps, &ok, o->tiles_left);
-	c.tick(0);
 	if (!ok || c.failed())
 		return false;
 	o->right = extend_dir(c, back, FWD, &psize, right, ps, &ok, o->tiles_right);
-	c.tick(1);
 	if (!ok || c.failed())
 		return false;
 	o->psize = psize;
@@ -1187,11 +1184,9 @@ ABB_HD bool walk_read(Ctx& c, const uint8_t* read_ascii, unsigned L, Emit& emit)
 		ContigOut o;
 		if (!extend_seed(c, rv, ps, &o) || c.failed())
 			return false;
-		c.tick(2);
 		if (!o.tip)
 			emit(c, i, o);
 		c.mark_covered(ps, rh, cov, nk, o, read_ascii, i);
-		c.tick(3);
 	}
 	return !c.failed();
 }

@@ -20,7 +20,6 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
-#include <chrono>
 #include <condition_variable>
 #include <deque>
 #include <map>
@@ -531,21 +530,16 @@ class BatchStream {
 		for (auto& w : m_workers)
 			w.join();
 		m_stitcher.join();
-		if (getenv("ABB_STREAM_STATS"))
-			fprintf(stderr, "BatchStream: consumer waited %.3f s, stitched %.3f s; reader read %.3f s, blocked %.3f s\n", m_tWait, m_tAppend,
-			        m_tRead, m_tThrottle);
 	}
 	/** next batch (owned by the stream, valid until the following call), nullptr at the end */
 	const ReadBatch* next()
 	{
-		const auto w0 = std::chrono::steady_clock::now();
 		std::unique_lock<std::mutex> l(m_mu);
 		if (m_given) {
 			m_outFree.push_back(std::move(m_given));
 			m_cv.notify_all();
 		}
 		m_cv.wait(l, [&] { return !m_outQ.empty() || m_stitchDone; });
-		m_tWait += std::chrono::duration<double>(std::chrono::steady_clock::now() - w0).count();
 		if (m_outQ.empty())
 			return nullptr;
 		m_given = std::move(m_outQ.front());
@@ -628,9 +622,7 @@ class BatchStream {
 					out->offsets.reserve(std::min<size_t>(want + 1, cap / 8));
 					out->id_offsets.reserve(std::min<size_t>(want + 1, cap / 8));
 				}
-				const auto a0 = std::chrono::steady_clock::now();
 				append(*m_cur, m_curPos, take);
-				m_tAppend += std::chrono::duration<double>(std::chrono::steady_clock::now() - a0).count();
 				m_curPos += take;
 			}
 			if (out->size()) {
@@ -677,10 +669,8 @@ class BatchStream {
 	/** wait until fewer than m_maxInFlight pieces are queued or parsed-but-unconsumed; false when stopping */
 	bool throttle()
 	{
-		const auto t0 = std::chrono::steady_clock::now();
 		std::unique_lock<std::mutex> l(m_mu);
 		m_cv.wait(l, [&] { return m_stop || m_nextSeq - m_nextOut < m_maxInFlight; });
-		m_tThrottle += std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
 		return !m_stop;
 	}
 	void work()
@@ -856,15 +846,11 @@ class BatchStream {
 	}
 	bool read_file(const std::string& path)
 	{
-		const auto m0 = std::chrono::steady_clock::now();
 		const int mapped = read_file_mapped(path);
-		if (mapped) {
-			m_tRead += std::chrono::duration<double>(std::chrono::steady_clock::now() - m0).count();
+		if (mapped)
 			return mapped > 0;
-		}
 		bool is_pipe = false;
 		FILE* f = open_input(path, &is_pipe);
-		const auto r0 = std::chrono::steady_clock::now();
 		RawBuf carry = take_buf(); // bytes read but not yet handed out
 		uint64_t line = 0;
 		char mode = 0;
@@ -936,7 +922,6 @@ class BatchStream {
 			m_cv.notify_all();
 		}
 		close_input(f, is_pipe, path);
-		m_tRead += std::chrono::duration<double>(std::chrono::steady_clock::now() - r0).count();
 		return ok;
 	}
 
@@ -965,7 +950,6 @@ class BatchStream {
 	std::unique_ptr<ReadBatch> m_given;               // the batch the caller holds
 	bool m_stitchDone = false;
 	std::thread m_stitcher;
-	double m_tWait = 0, m_tAppend = 0, m_tRead = 0, m_tThrottle = 0;
 };
 
 /** SIToBytes (Common/StringUtil.h:181-219): number with optional k/M/G suffix (powers of 1024) */

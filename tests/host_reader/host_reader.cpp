@@ -5,6 +5,7 @@
 // Both print "id<TAB>sequence" per read and a "# batch N" line per batch (stream mode), so that the
 // test can compare the two record for record and check the batch sizes.
 #include "../../abyss_b200/host/reads.h"
+#include <chrono>
 
 int main(int argc, char** argv)
 {

@@ -88,7 +88,6 @@ struct HostCtx {
 	uint32_t tile_index(const TileRec* t) const { return (uint32_t)(t - tile_recs.data()); }
 	const TileRec* tile_at(uint32_t idx) const { return &tile_recs[idx]; }
 	void prefetch(const void*) const {}
-	void tick(int) {}
 	void wr32(uint32_t* p, uint32_t v) { *p = v; }
 	uint64_t rd64(const uint64_t* p) { return *p; }
 	void wr64(uint64_t* p, uint64_t v) { *p = v; }

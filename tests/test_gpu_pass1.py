@@ -79,6 +79,42 @@ def test_hash_reads_vs_oracle_many_k(abb, oracle, k):
     assert (rh == np.concatenate(eh)).all()
 
 
+@pytest.mark.parametrize("mask", ["", "".join("0" if i % 7 == 3 else "1" for i in range(31))])
+def test_hash_reads_dev_unaligned_bases(abb, mask):
+    # device-resident reads at 0, 1, 7 and 15 bytes past an aligned address: the bulk copy that stages read blocks needs a
+    # 16-byte aligned source, so the unaligned batches are hashed from global memory and must give the same windows
+    import torch
+    from abyss_b200.capi import pack_reads
+    k = 31
+    rng = np.random.default_rng(17)
+    seqs = []
+    for i in range(300):
+        s = rng.choice(list("ACGT"), size=int(rng.integers(0, 400)))
+        if i % 4 == 0 and len(s):
+            s[rng.integers(0, len(s), size=max(1, len(s) // 40))] = "N"
+        seqs.append("".join(s))
+    seqs.insert(150, "".join(rng.choice(list("ACGT"), size=9000)))  # longer than a staging buffer
+    h0_ref, valid_ref, slot_offs = abb.hash_reads(k, seqs, mask)
+    total = int(slot_offs[-1])
+    bases, offs = pack_reads(seqs)
+    dev = torch.device("cuda", 0)
+    buf = torch.zeros(len(bases) + 32, dtype=torch.uint8, device=dev)
+    assert buf.data_ptr() % 16 == 0
+    d_offs = torch.from_numpy(offs.astype(np.int64)).to(dev)
+    f = abb.Filter.counting(4096, 4, k, mask=mask)
+    for off in (0, 1, 7, 15):
+        buf.zero_()
+        buf[off:off + len(bases)] = torch.from_numpy(bases).to(dev)
+        h0 = torch.full((total,), -1, dtype=torch.int64, device=dev)
+        valid = torch.full((total,), 7, dtype=torch.uint8, device=dev)
+        torch.cuda.synchronize(dev)
+        n = f.hash_reads_dev(buf.data_ptr() + off, d_offs.data_ptr(), len(seqs), h0.data_ptr(), valid.data_ptr(), total)
+        assert n == total
+        assert (h0.cpu().numpy().view(np.uint64) == h0_ref).all(), off
+        assert (valid.cpu().numpy() == valid_ref).all(), off
+    f.close()
+
+
 def test_counting_fixtures(abb, golden_dir):
     reads60 = seeded(11, 3000, 1500, 60)
     reads150 = seeded(12, 20000, 600, 150)

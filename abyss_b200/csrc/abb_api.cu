@@ -57,7 +57,7 @@ static FilterView view_of(const abb_filter* f)
 {
 	FilterView v;
 	v.data = f->d_data.p;
-	v.level_stride = f->bytes_per_level;
+	v.level_stride = f->level_stride();
 	v.levels = f->levels;
 	return v;
 }
@@ -820,8 +820,8 @@ static int alloc_filter(std::unique_ptr<abb_filter> f, abb_filter** out)
 	ABB_CUDA(cudaEventCreate(f->ev0.out()));
 	ABB_CUDA(cudaEventCreate(f->ev1.out()));
 	// slack: the in-place all-gather of position shards rounds each shard up to 16 bytes (abb_filter_allgather)
-	ABB_CHECK(f->d_data.alloc(f->bytes_per_level * levels + 4096));
-	ABB_CUDA(cudaMemsetAsync(f->d_data.p, 0, f->bytes_per_level * levels, f->stream));
+	ABB_CHECK(f->d_data.alloc(f->level_stride() * levels + 4096));
+	ABB_CUDA(cudaMemsetAsync(f->d_data.p, 0, f->level_stride() * levels, f->stream));
 	ABB_CHECK(f->d_ctl.alloc(8));
 	ABB_CUDA(cudaMemsetAsync(f->d_ctl.p, 0, 8 * sizeof(unsigned), f->stream));
 	ABB_CHECK(f->d_stats.alloc(8));
@@ -1233,7 +1233,7 @@ void* abb_filter_device_ptr(abb_filter* f, int level)
 		return nullptr;
 	cudaSetDevice(f->device);
 	cudaStreamSynchronize(f->stream);
-	return f->d_data.p + (uint64_t)level * f->bytes_per_level;
+	return f->level_data((unsigned)level);
 }
 
 static int query_hashes(abb_filter* f, const uint64_t* hashes, uint64_t n, uint8_t* out, bool want_min)
@@ -1407,7 +1407,7 @@ static int level_ptr(abb_filter* f, int level, uint64_t nbytes, uint8_t** p)
 	ABB_REQUIRE((unsigned)level < f->levels, "level %d out of range", level);
 	ABB_REQUIRE(nbytes == f->bytes_per_level, "buffer is %llu bytes, the filter level is %llu", (unsigned long long)nbytes,
 	            (unsigned long long)f->bytes_per_level);
-	*p = f->d_data.p + (uint64_t)level * f->bytes_per_level;
+	*p = f->level_data((unsigned)level);
 	return ABB_OK;
 }
 
@@ -1437,7 +1437,7 @@ int abb_filter_clear(abb_filter* f)
 {
 	ABB_REQUIRE(f, "NULL filter");
 	ABB_CUDA(cudaSetDevice(f->device));
-	ABB_CUDA(cudaMemsetAsync(f->d_data.p, 0, f->bytes_per_level * f->levels, f->stream));
+	ABB_CUDA(cudaMemsetAsync(f->d_data.p, 0, f->level_stride() * f->levels, f->stream));
 	ABB_CUDA(cudaStreamSynchronize(f->stream));
 	return ABB_OK;
 }
@@ -1457,7 +1457,7 @@ int abb_filter_popcount(abb_filter* f, uint64_t* nonzero, uint64_t* at_or_above_
 	ABB_CUDA(cudaSetDevice(f->device));
 	ABB_CUDA(cudaMemsetAsync(f->d_stats.p + 4, 0, 2 * sizeof(unsigned long long), f->stream));
 	// bit / cascading: population of the LAST level (the one contains() consults)
-	const uint8_t* p = f->d_data.p + (uint64_t)(f->levels - 1) * f->bytes_per_level;
+	const uint8_t* p = f->level_data(f->levels - 1);
 	k_popcount<<<sm_count() * 8, 256, 0, f->stream>>>(p, f->bytes_per_level, f->kind == ABB_COUNTING, f->threshold, f->d_stats.p + 4);
 	f->st.launches += 1;
 	ABB_CUDA(cudaGetLastError());

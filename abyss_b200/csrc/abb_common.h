@@ -204,6 +204,12 @@ struct abb_filter {
 	abb::DevBuf<unsigned> gq_len;
 	abb::DevBuf<uint64_t> gq_self;
 
+	/** device bytes from one level to the next.  Bit and cascading levels start on 16-byte boundaries: bits_set ORs 4-byte words
+	 *  and k_popcount loads uint4, while size / 8 need only be a multiple of 1.  Counting filters have one level, and the
+	 *  Konnector kernels address a packed array of levels.  The padding is never part of a level: bytes_per_level is. */
+	uint64_t level_stride() const { return kind == ABB_BIT || kind == ABB_CASCADING ? (bytes_per_level + 15) & ~15ULL : bytes_per_level; }
+	uint8_t* level_data(unsigned level) const { return d_data.p + (uint64_t)level * level_stride(); }
+
 	// statistics
 	abb_insert_stats st = {};
 	bool profile = false; // time the k_window launches with CUDA events (every prof_stride-th window)

@@ -93,7 +93,7 @@ int abb_filter_read_bits(abb_filter* f, int level, const uint8_t* host, uint64_t
 	ABB_CUDA(cudaMemcpyAsync(src.p, host, nbytes, cudaMemcpyHostToDevice, f->stream));
 	const uint64_t dest_bytes = bit_offset / 8 + nbytes + 1;
 	k_kon_read_bits<<<std::min<unsigned>(blocks_for(dest_bytes, 256), sm_count() * 16), 256, 0, f->stream>>>(
-	    f->d_data.p + (uint64_t)level * f->bytes_per_level, f->bytes_per_level, src.p, bits, bit_offset, op);
+	    f->level_data((unsigned)level), f->bytes_per_level, src.p, bits, bit_offset, op);
 	f->st.launches += 1;
 	ABB_CUDA(cudaGetLastError());
 	ABB_CUDA(cudaStreamSynchronize(f->stream));
@@ -110,7 +110,7 @@ int abb_filter_level_popcount(abb_filter* f, int level, uint64_t* n)
 	ABB_CUDA(cudaSetDevice(f->device));
 	unsigned long long* d_n = f->d_stats.p + 6;
 	ABB_CUDA(cudaMemsetAsync(d_n, 0, sizeof(unsigned long long), f->stream));
-	k_kon_popcount<<<sm_count() * 8, 256, 0, f->stream>>>(f->d_data.p + (uint64_t)level * f->bytes_per_level, f->bytes_per_level, d_n);
+	k_kon_popcount<<<sm_count() * 8, 256, 0, f->stream>>>(f->level_data((unsigned)level), f->bytes_per_level, d_n);
 	f->st.launches += 1;
 	ABB_CUDA(cudaGetLastError());
 	unsigned long long h = 0;
@@ -134,7 +134,7 @@ int abb_filter_compare(abb_filter* a, abb_filter* b, uint64_t counts[4])
 	ABB_CUDA(cudaMemsetAsync(d_c, 0, 3 * sizeof(unsigned long long), a->stream));
 	const uint64_t nbytes = a->bytes_per_level;
 	k_kon_compare<<<std::min<unsigned>(blocks_for(nbytes, 256), sm_count() * 8), 256, 0, a->stream>>>(
-	    a->d_data.p + (uint64_t)(a->levels - 1) * nbytes, b->d_data.p + (uint64_t)(b->levels - 1) * nbytes, nbytes, d_c);
+	    a->level_data(a->levels - 1), b->level_data(b->levels - 1), nbytes, d_c);
 	a->st.launches += 1;
 	ABB_CUDA(cudaGetLastError());
 	unsigned long long h[3] = { 0, 0, 0 };

@@ -118,6 +118,20 @@ def test_abyss_bloom_build_and_prebuilt(cases):
     assert hashlib.sha256(open(rh, "rb").read()).hexdigest() == c["rolling_hash_l2_file_sha256"]
 
 
+def test_rolling_hash_levels_not_multiple_of_16_bytes(cases):
+    # -b 1000 over two levels: each level rounds up to 504 bytes, not a multiple of 16, and -v reports the population of
+    # the last one; file identical to the reference's (tests/golden/make_golden_hashnum.py)
+    g = json.load(open(os.path.join(ROOT, "tests", "golden", "hashnum_cases.json")))["rolling_hash"]
+    c, fq, d = cases[g["reads"]]
+    rh = str(d / "rh_b1000.bloom")
+    r = subprocess.run([os.path.join(BIN, "abyss-bloom"), "build", "-k", str(c["k"]), "-t", "rolling-hash", "-l", str(g["levels"]),
+                        f"-H{g['H']}", f"-b{g['b']}", "-v", rh, fq], capture_output=True, text=True)
+    assert r.returncode == 0, r.stderr
+    blob = open(rh, "rb").read()
+    assert len(blob) == g["file_bytes"]
+    assert hashlib.sha256(blob).hexdigest() == g["file_sha256"]
+
+
 def test_cli_errors(cases):
     c, fq, d = cases["e2e_g20k_k32"]
     exe = os.path.join(BIN, "abyss-bloom-dbg")

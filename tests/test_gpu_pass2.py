@@ -137,3 +137,39 @@ def test_assembler_reset_reuses_handle(abb, golden_dir):
     a.close()
     f.close()
     assert outs[0] == outs[1] == open(os.path.join(golden_dir, "e2e_g20k_k32.fa")).read()
+
+
+HASHNUM = json.load(open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "hashnum_cases.json")))
+
+
+@pytest.mark.parametrize("case", HASHNUM["dbg"], ids=lambda c: c["name"])
+def test_hash_counts_identical_to_reference(abb, golden_dir, tmp_path, case):
+    # H = 1, 2, 5, 8, 9: the MAXH = 4 kernels with lanes that have nothing to probe, and the MAXH = 8 and 32 kernels.  Counters,
+    # FASTA and read log against the reference's -j1 run (tests/golden/make_golden_hashnum.py), through the C ABI as one batch
+    # and in batches of 997 reads, and through abyss-bloom-dbg
+    import hashlib
+    import subprocess
+    from abyss_b200.capi import fixed_length_reads, bloom_dbg, READ_CODES, Filter
+    c, rs = load_case(golden_dir, case["reads"])
+    H = case["H"]
+    ids = [rs.read_id(i) for i in range(rs.n)]
+    reads = fixed_length_reads(rs.ascii(0, rs.n))
+    f = Filter.counting(c["counters"], H, c["k"], c["kc"])
+    f.insert_reads(reads)
+    assert hashlib.sha256(f.download().tobytes()).hexdigest() == case["counters_sha256"]
+    f.close()
+    md5 = lambda b: hashlib.md5(b).hexdigest()  # noqa: E731
+    for batch in (None, 997):
+        fasta, codes = bloom_dbg(ids, reads, c["k"], c["kc"], H, counters=c["counters"], batch_reads=batch, read_log=True)
+        log = "read_id\tresult\n" + "".join(f"{ids[i]}\t{READ_CODES[codes[i]]}\n" for i in range(rs.n))
+        assert fasta.count(">") == case["n_contigs"], batch
+        assert md5(fasta.encode()) == case["fasta_md5"], batch
+        assert md5(log.encode()) == case["readlog_md5"], batch
+    fq, fa, log = (str(tmp_path / x) for x in ("reads.fq", "out.fa", "readlog.tsv"))
+    rs.write_fastq(fq)
+    exe = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "abyss_b200", "lib", "abyss-bloom-dbg")
+    r = subprocess.run([exe, f"-k{c['k']}", f"--kc={c['kc']}", f"-b{c['b']}", f"-H{H}", "-j1", f"--read-log={log}", "-o", fa, fq],
+                       capture_output=True, text=True)
+    assert r.returncode == 0, r.stderr
+    assert md5(open(fa, "rb").read()) == case["fasta_md5"]
+    assert md5(open(log, "rb").read()) == case["readlog_md5"]

@@ -21,7 +21,7 @@ SOURCES = {
     "abb_api.cu": ["abb_common.h", "abb_device.cuh", "abb_insert.cuh", "abb_shard.cuh", "abb_graph.cuh", "../../include/abyss_b200.h"],
     "abb_assemble.cu": ["abb_common.h", "abb_device.cuh", "abb_walk.cuh", "../../include/abyss_b200.h"],
     "abb_overlap.cu": ["abb_common.h", "abb_device.cuh", "abb_overlap.cuh", "../../include/abyss_b200.h"],
-    "abb_konnector.cu": ["abb_common.h", "abb_device.cuh", "abb_konnector.cuh", "../../include/abyss_b200.h"],
+    "abb_konnector.cu": ["abb_common.h", "abb_device.cuh", "abb_konnector.cuh", "abb_walk.cuh", "../../include/abyss_b200.h"],
 }
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = [

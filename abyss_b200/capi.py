@@ -139,6 +139,7 @@ SIGNATURES = {
     "abb_filter_set_profiling": (C.c_int, [_vp, C.c_int]),
     "abb_filter_stream": (_vp, [_vp]),
     "abb_contains_reads": (C.c_int, [_vp, _vp, _vp, C.c_uint64, _vp, _vp, C.c_uint64, _u64p]),
+    "abb_trim_reads": (C.c_int, [_vp, _vp, _vp, C.c_uint64, C.c_uint, _vp, _vp]),
     "abb_successors": (C.c_int, [_vp, _vp, C.c_uint64, C.c_uint, _vp, _vp, _vp]),
     "abb_overlap_create": (C.c_int, [C.POINTER(_vp), C.c_int]),
     "abb_overlap_destroy": (C.c_int, [_vp]),
@@ -284,6 +285,15 @@ class Filter:
         n = C.c_uint64(0)
         check(self._lib.abb_filter_level_popcount(self._h, level, C.byref(n)))
         return n.value
+
+    def trim_reads(self, seqs_or_arrays, min_branch_len: int) -> tuple[np.ndarray, np.ndarray]:
+        """`abyss-bloom trim`: per read, the bases to cut from the left and from the right end (calcLeftTrim of the read and of
+        its reverse complement, Bloom/bloom.cc:1236-1290); Konnector filters only"""
+        bases, offs = seqs_or_arrays if isinstance(seqs_or_arrays, tuple) else pack_reads(seqs_or_arrays)
+        n = len(offs) - 1
+        left, right = np.zeros(n, dtype=np.uint32), np.zeros(n, dtype=np.uint32)
+        check(self._lib.abb_trim_reads(self._h, _ptr(bases), _ptr(offs), n, min_branch_len, _ptr(left), _ptr(right)))
+        return left, right
 
     @classmethod
     def counting(cls, counters, num_hashes, k, threshold=0, mask="", device=0):

@@ -198,6 +198,10 @@ struct abb_filter {
 	abb::DevBuf<uint8_t> bases;
 	abb::DevBuf<uint64_t> offs, slot_offs, h0, lit, bounds;
 	abb::DevBuf<uint8_t> valid, scan_tmp, out8, sh_buf;
+	// abb_trim_reads: the batch, its trim lengths and the walk scratch of the grid, kept from one batch to the next
+	abb::DevBuf<uint8_t> trim_bases, trim_scratch;
+	abb::DevBuf<uint64_t> trim_offs;
+	abb::DevBuf<uint32_t> trim_out;
 	// abb_successors staging (a graph dump issues thousands of small queries: no allocation per call)
 	abb::DevBuf<uint8_t> gq_kmers;
 	abb::DevBuf<abb_succ_info> gq_info;

@@ -120,6 +120,57 @@ int abb_filter_level_popcount(abb_filter* f, int level, uint64_t* n)
 	return ABB_OK;
 }
 
+int abb_trim_reads(abb_filter* f, const char* bases, const uint64_t* offsets, uint64_t n_reads, unsigned min_branch_len, uint32_t* left,
+                   uint32_t* right)
+{
+	ABB_REQUIRE(f, "NULL filter");
+	if (f->kind != ABB_KONNECTOR) {
+		set_error("abb_trim_reads: only Konnector (-t konnector) filters have the trim graph");
+		return ABB_ESTATE;
+	}
+	if (n_reads == 0)
+		return ABB_OK;
+	ABB_REQUIRE(bases && offsets && left && right, "NULL buffer");
+	ABB_REQUIRE(offsets[0] == 0, "offsets[0] must be 0");
+	ABB_REQUIRE(f->k >= 2, "k must be at least 2");
+	for (uint64_t r = 0; r < n_reads; ++r)
+		ABB_REQUIRE(offsets[r + 1] - offsets[r] < (1ULL << 31), "read %llu is too long", (unsigned long long)r);
+	ABB_CUDA(cudaSetDevice(f->device));
+	const uint64_t n_bases = offsets[n_reads];
+	int per_sm = 0; // a grid that is resident all at once: the walk scratch is sized per warp of the grid
+	ABB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_kon_trim, kKonTrimThreads, 0));
+	const unsigned blocks =
+	    (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(blocks_for(2 * n_reads * 32, kKonTrimThreads), (uint64_t)sm_count() * std::max(per_sm, 1)));
+	const uint64_t n_warps = (uint64_t)blocks * kKonTrimThreads / 32;
+	DevBuf<uint8_t>& d_bases = f->trim_bases;
+	DevBuf<uint64_t>& d_offs = f->trim_offs;
+	DevBuf<uint32_t>& d_out = f->trim_out;
+	const size_t frame_bytes = n_warps * kFrameCap * sizeof(Frame);
+	ABB_CHECK(d_bases.reserve(n_bases + 16));
+	ABB_CHECK(d_offs.reserve(n_reads + 1));
+	ABB_CHECK(f->trim_scratch.reserve(frame_bytes + n_warps * kLookCap * sizeof(uint64_t)));
+	ABB_CHECK(d_out.reserve(2 * n_reads));
+	Frame* d_frames = reinterpret_cast<Frame*>(f->trim_scratch.p);
+	uint64_t* d_look = reinterpret_cast<uint64_t*>(f->trim_scratch.p + frame_bytes);
+	const SyncOnExit sync = { f->stream };
+	ABB_CUDA(cudaMemcpyAsync(d_bases.p, bases, n_bases, cudaMemcpyHostToDevice, f->stream));
+	ABB_CUDA(cudaMemcpyAsync(d_offs.p, offsets, (n_reads + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, f->stream));
+	k_kon_trim<<<blocks, kKonTrimThreads, 0, f->stream>>>(d_bases.p, d_offs.p, n_reads, kon_geom(f->k), kon_view(f), min_branch_len, d_frames,
+	                                                      d_look, d_out.p, d_out.p + n_reads);
+	ABB_CUDA(cudaGetLastError());
+	f->st.launches += 1;
+	ABB_CUDA(cudaMemcpyAsync(left, d_out.p, n_reads * sizeof(uint32_t), cudaMemcpyDeviceToHost, f->stream));
+	ABB_CUDA(cudaMemcpyAsync(right, d_out.p + n_reads, n_reads * sizeof(uint32_t), cudaMemcpyDeviceToHost, f->stream));
+	ABB_CUDA(cudaStreamSynchronize(f->stream));
+	for (uint64_t r = 0; r < n_reads; ++r)
+		if (left[r] == kKonTrimFailed || right[r] == kKonTrimFailed) {
+			set_error("abb_trim_reads: read %llu of the batch: the branch search outgrew its scratch (%u frames, %u visited vertices)",
+			          (unsigned long long)r, kFrameCap, kLookCap);
+			return ABB_ESTATE;
+		}
+	return ABB_OK;
+}
+
 int abb_filter_compare(abb_filter* a, abb_filter* b, uint64_t counts[4])
 {
 	ABB_REQUIRE(a && b && counts, "NULL argument");

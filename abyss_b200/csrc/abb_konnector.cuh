@@ -8,6 +8,7 @@
 // k-mer is byte 7 - j%8 of word j/8 and the byte string CityHash reads is the words' big-endian image.
 #pragma once
 #include "abb_device.cuh"
+#include "abb_walk.cuh"
 
 namespace abb {
 
@@ -274,6 +275,153 @@ ABB_HD uint8_t kon_copy_bits_byte(uint8_t old, const uint8_t* src, uint64_t bits
 	return (uint8_t)(v & 0xFF);
 }
 
+// ---- the Konnector de Bruijn graph (Konnector/DBGBloom.h) and `abyss-bloom trim` (Bloom/bloom.cc:1233-1382) -------------
+/** One step of a k-mer in place: FWD drops base 0 and appends b (Kmer::shift(SENSE) + setLastBase), REV drops base k-1 and
+ *  prepends b; both images follow.  A step to the left of the forward image is a step to the right of the reverse
+ *  complement with the complementary base, so one shift serves both directions.  Only the words that k uses are shifted:
+ *  a step sits on the critical path of every graph move, where kon_push (a bulk scan) shifts all six. */
+ABB_HD void kon_step(KonKmer& m, const KonGeom& g, Dir d, unsigned b)
+{
+	if (d == REV) {
+KON_UNROLL
+		for (unsigned j = 0; j < kKonWords; ++j) {
+			const uint64_t t = m.f[j];
+			m.f[j] = m.r[j];
+			m.r[j] = t;
+		}
+		b = 3 - b;
+	}
+KON_UNROLL
+	for (unsigned j = 0; j < kKonWords; ++j) { // shift left one base, b goes to position k-1
+		if (j > g.last_word)
+			break;
+		m.f[j] = (m.f[j] << 2) | (j + 1 < kKonWords && j < g.last_word ? m.f[j + 1 < kKonWords ? j + 1 : j] >> 62 : 0);
+		if (j == g.last_word)
+			m.f[j] |= (uint64_t)b << g.last_shift;
+	}
+KON_UNROLL
+	for (int j = kKonWords - 1; j >= 0; --j) { // shift right one base, the complement goes to position 0
+		if ((unsigned)j > g.last_word)
+			continue;
+		m.r[j] = (m.r[j] >> 2) | (j > 0 ? m.r[j > 0 ? j - 1 : 0] << 62 : 0);
+		if ((unsigned)j == g.last_word)
+			m.r[j] &= g.last_mask;
+	}
+	m.r[0] |= (uint64_t)(3 - b) << 62;
+	if (d == REV) {
+KON_UNROLL
+		for (unsigned j = 0; j < kKonWords; ++j) {
+			const uint64_t t = m.f[j];
+			m.f[j] = m.r[j];
+			m.r[j] = t;
+		}
+	}
+}
+
+/** A vertex of DBGBloom: a k-mer AS GIVEN, not up to reverse complement (graph_traits<DBGBloom>::vertex_descriptor is Kmer,
+ *  whose operator== compares the packed bytes), so `visited` in lookAhead / trueBranch and "source(*iei) == u" tell a k-mer
+ *  from its reverse complement.  id stands for the forward image in those comparisons: the image itself for k <= 32
+ *  (exact), a chain of CityHash's 128-to-64-bit mix over its words above that.  A walk compares a vertex with at most
+ *  kFrameCap + kLookCap others, all within a few dozen steps of one read k-mer; two different k-mers among them sharing
+ *  the 64-bit mix is a ~2^-64 event per comparison, the same order as the ntHash identity of the pass-2 walk. */
+struct KonVtx {
+	KonKmer m;
+	uint64_t id;
+	ABB_HD uint64_t canon() const { return id; }
+};
+ABB_HD uint64_t kon_identity(const KonKmer& m, const KonGeom& g)
+{
+	uint64_t id = m.f[0];
+KON_UNROLL
+	for (unsigned j = 1; j < kKonWords; ++j) {
+		if (j > g.last_word)
+			break;
+		id = city_hash16(id, m.f[j]);
+	}
+	return id;
+}
+/** the vertex interface of the walk templates (abb_walk.cuh); returns the base that fell off */
+ABB_HD unsigned vtx_step(KonVtx& v, unsigned, const KonGeom& g, Dir d, unsigned b)
+{
+	const unsigned out = d == FWD ? (unsigned)(v.m.f[0] >> 62) : 3u - (unsigned)(v.m.r[0] >> 62);
+	kon_step(v.m, g, d, b);
+	v.id = kon_identity(v.m, g);
+	return out;
+}
+ABB_HD void vtx_unstep(KonVtx& v, unsigned k, const KonGeom& g, Dir d, unsigned out) { vtx_step(v, k, g, opposite(d), out); }
+
+/** Bloom::hash of neighbour n of m: n = 0..3 the out-edges (append A, C, G, T: out_edge_iterator, DBGBloom.h:160-221),
+ *  4..7 the in-edges (prepend A, C, G, T: in_edge_iterator, :224-285), 8 the k-mer itself */
+ABB_HD uint64_t kon_neighbor_hash(const KonKmer& m, const KonGeom& g, uint64_t seed, unsigned n)
+{
+	KonKmer t = m;
+	if (n < 8)
+		kon_step(t, g, n < 4 ? FWD : REV, n & 3);
+	return kon_hash(t, g, seed);
+}
+/** BloomFilter::operator[] on the last level: the level a cascading build writes to its file (vertex_exists, DBGBloom.h:294-299) */
+ABB_HD bool kon_test(const KonView& fv, uint64_t hash)
+{
+	const uint64_t pos = fastmod_u64(hash, fv.full);
+	if (pos < fv.start || pos - fv.start >= fv.bits)
+		return false;
+	const uint64_t bit = pos - fv.start;
+	const uint8_t* level = fv.data + (uint64_t)(fv.levels - 1) * fv.bytes_per_level;
+	return (level[bit / 8] >> (7 - bit % 8)) & 1;
+}
+
+constexpr uint32_t kKonTrimFailed = 0xffffffffu; // the walk scratch overflowed: no trim length for this task
+
+/**
+ * calcLeftTrim (bloom.cc:1236-1290) of seq[0, len), len >= k, or of its reverse complement (rc: read from the end of the
+ * read, never materialised).  KmerIterator (Common/KmerIterator.h) skips the windows that hold a non-ACGT character; a
+ * k-mer that is not in the filter is skipped; the first k-mer that is must be a tip -- (DEAD_END, LENGTH_LIMIT) or the
+ * reverse -- for the scan to go on, and a later one stops it when either side is AMBI_OUT.  Stopping at window p gives
+ * p == 0 ? 0 : k + p - 1.  When the scan runs off the end the reference's pos() is SIZE_MAX and its int result k - 2: kept.
+ *
+ * Ctx is the walk context of abb_walk.cuh (k, trim = minBranchLen, rt = the KonGeom, neighbors / neighbors_dir, the scratch
+ * accessors) plus
+ *   unsigned neighbors_self(const KonVtx&)   neighbors() with bit 8 = the k-mer itself is in the filter: nine probes issued
+ *                                            together, so a window costs one memory round trip whether or not it is a vertex
+ *   unsigned char base(const uint8_t* seq, unsigned len, unsigned i)   seq[i]
+ */
+template <class Ctx>
+ABB_HD uint32_t kon_left_trim(Ctx& c, const uint8_t* seq, unsigned len, bool rc)
+{
+	const unsigned k = c.k;
+	KonVtx v;
+	kon_clear(v.m);
+	unsigned run = 0;
+	bool first = true;
+	for (unsigned i = 0; i < len; ++i) {
+		unsigned code = base_code(c.base(seq, len, rc ? len - 1 - i : i));
+		if (code > 3) { // the next k-mer starts after this character; the k bases pushed by then overwrite every position
+			run = 0;
+			continue;
+		}
+		kon_step(v.m, c.rt, FWD, rc ? 3 - code : code);
+		if (++run < k)
+			continue;
+		const unsigned nb = c.neighbors_self(v);
+		if (!(nb & 256u))
+			continue;
+		v.id = kon_identity(v.m, c.rt);
+		unsigned vbase = 0;
+		const ExtCode left = successor(c, v, nb & 255u, REV, &vbase);
+		const ExtCode right = successor(c, v, nb & 255u, FWD, &vbase);
+		if (c.failed())
+			return kKonTrimFailed;
+		const bool stop = first ? !((left == ER_DEAD_END && right == ER_LENGTH_LIMIT) || (left == ER_LENGTH_LIMIT && right == ER_DEAD_END))
+		                        : (left == ER_AMBI_OUT || right == ER_AMBI_OUT); // this successor never returns AMBI_IN
+		if (stop) {
+			const unsigned pos = i + 1 - k;
+			return pos == 0 ? 0 : k + pos - 1;
+		}
+		first = false;
+	}
+	return k - 2;
+}
+
 #if defined(__CUDACC__)
 // ---- kernels -----------------------------------------------------------------------------------------------------------
 constexpr unsigned kKonSlotsPerThread = 128; // windows one thread rolls through (the first k - 1 bases are the overhead)
@@ -413,6 +561,94 @@ __global__ void k_kon_compare(const uint8_t* __restrict__ a, const uint8_t* __re
 		atomicAdd(out + 0, n11);
 		atomicAdd(out + 1, n10);
 		atomicAdd(out + 2, n01);
+	}
+}
+
+/** The walk context of one warp on a Konnector filter.  All 32 lanes run the graph logic with the same arguments; they part
+ *  only in the probes, where lane n < 9 hashes neighbour n (kon_neighbor_hash) and loads its bit, and in the scratch
+ *  accessors.  The scratch conventions are WarpCtx's (abb_assemble.cu): every lane stores the same value and reads back
+ *  its own store. */
+struct KonWarpCtx {
+	unsigned k, trim;
+	KonGeom rt;
+	KonView fv;
+	unsigned lane;
+	Frame* frames;
+	uint64_t* look;
+	unsigned fail_;
+	unsigned chunk;       // which 32 characters of the read `held` is
+	unsigned char held;   // character 32 * chunk + lane
+
+	__device__ unsigned probe(const KonVtx& v, unsigned lanes) const
+	{
+		bool ok = false;
+		if ((lanes >> lane) & 1u)
+			ok = kon_test(fv, kon_neighbor_hash(v.m, rt, fv.seed, lane));
+		return __ballot_sync(0xffffffffu, ok);
+	}
+	__device__ unsigned neighbors_self(const KonVtx& v) const { return probe(v, 0x1ffu); }
+	__device__ unsigned neighbors(const KonVtx& v) const { return probe(v, 0xffu); }
+	__device__ unsigned neighbors_dir(const KonVtx& v, Dir d) const { return d == FWD ? probe(v, 0x0fu) : probe(v, 0xf0u) >> 4; }
+	/** seq[i]: the warp keeps 32 characters in registers (one coalesced load per 32 windows instead of one load per window) */
+	__device__ unsigned char base(const uint8_t* seq, unsigned len, unsigned i)
+	{
+		if (i / 32 != chunk) {
+			chunk = i / 32;
+			const unsigned j = chunk * 32 + lane;
+			held = j < len ? seq[j] : 0;
+		}
+		return (unsigned char)__shfl_sync(0xffffffffu, (unsigned)held, i % 32);
+	}
+	__device__ uint64_t rd64(const uint64_t* p) const { return *(const volatile uint64_t*)p; }
+	__device__ void wr64(uint64_t* p, uint64_t v) const { *(volatile uint64_t*)p = v; }
+	__device__ void sync() const { __syncwarp(); }
+	__device__ bool find64(const uint64_t* a, unsigned n, uint64_t key, unsigned stride) const
+	{
+		for (unsigned b0 = 0; b0 < n; b0 += 32) {
+			const unsigned i = b0 + lane;
+			const bool hit = i < n && *(const volatile uint64_t*)(a + (size_t)i * stride) == key;
+			if (__any_sync(0xffffffffu, hit))
+				return true;
+		}
+		return false;
+	}
+	__device__ void fail(unsigned why) { fail_ |= 1u << why; }
+	__device__ bool failed() const { return fail_ != 0; }
+};
+
+constexpr unsigned kKonTrimThreads = 128;
+
+/** `abyss-bloom trim`: task 2r is the left end of read r, task 2r + 1 its right end (the same scan over the reverse
+ *  complement); each writes one trim length, kKonTrimFailed when the walk scratch overflowed, 0 for a read shorter than k
+ *  (which the caller echoes).  One warp per task, tasks dealt round-robin to a grid that fills the device once: most tasks
+ *  end at their first window after one probe round, a few walk tens of windows with a trueBranch search at each, and with
+ *  hundreds of tasks per warp, the two ends of a read and neighbouring reads on different warps, the long ones spread out.
+ *  frames / look: kFrameCap / kLookCap entries per warp of the grid. */
+__global__ void __launch_bounds__(kKonTrimThreads) k_kon_trim(const uint8_t* __restrict__ bases, const uint64_t* __restrict__ offs,
+                                                             uint64_t n_reads, KonGeom g, KonView fv, unsigned min_branch_len,
+                                                             Frame* __restrict__ frames, uint64_t* __restrict__ look,
+                                                             uint32_t* __restrict__ left, uint32_t* __restrict__ right)
+{
+	const uint64_t warp = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) / 32, n_warps = (uint64_t)gridDim.x * blockDim.x / 32;
+	KonWarpCtx c;
+	c.k = g.k;
+	c.trim = min_branch_len;
+	c.rt = g;
+	c.fv = fv;
+	c.lane = threadIdx.x & 31;
+	c.frames = frames + warp * kFrameCap;
+	c.look = look + warp * kLookCap;
+	for (uint64_t t = warp; t < 2 * n_reads; t += n_warps) {
+		const uint64_t r = t / 2, b0 = offs[r], len = offs[r + 1] - b0;
+		uint32_t out = 0;
+		if (len >= g.k) {
+			c.fail_ = 0;
+			c.chunk = 0xffffffffu;
+			out = kon_left_trim(c, bases + b0, (unsigned)len, (t & 1) != 0);
+		}
+		if (c.lane == 0)
+			(t & 1 ? right : left)[r] = out;
+		__syncwarp();
 	}
 }
 #endif

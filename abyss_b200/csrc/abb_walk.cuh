@@ -388,19 +388,24 @@ ABB_HD unsigned ctz4(unsigned m) { return (m & 1) ? 0 : (m & 2) ? 1 : (m & 4) ? 
  *   uint32_t tile_index(const TileRec*); void wr32(uint32_t*, uint32_t)
  *   void mark_covered(ps, rh, cov, nk, contig)         cooperative: flag read k-mers that lie on the contig path
  *   Frame* frames; uint64_t* look;   per-warp scratch
+ *
+ * lookAhead / trueBranch / successor below are templates over the vertex type V as well: they reach a vertex only through
+ * vtx_step / vtx_unstep (found by argument-dependent lookup), V::canon() (vertex identity) and the context's neighbors*;
+ * `c.rt` is whatever the vertex's vtx_step takes as its third argument.  Vtx<KW> (ntHash, identity up to reverse
+ * complement) is the vertex of abyss-bloom-dbg; KonVtx (abb_konnector.cuh: exact, strand-specific) that of abyss-bloom trim.
  */
 
 // ------------------------------------------------------------------------------------------
 // lookAhead (Graph/ExtendPath.h:99-161): bounded DFS with a permanent visited set
 // ------------------------------------------------------------------------------------------
-template <int KW, class Ctx>
-ABB_HD bool look_ahead(Ctx& c, const Vtx<KW>& start, Dir dir, unsigned limit)
+template <class V, class Ctx>
+ABB_HD bool look_ahead(Ctx& c, const V& start, Dir dir, unsigned limit)
 {
 	unsigned nvis = 0;
 	c.wr64(c.look + nvis++, start.canon()); // visited.insert(u)
 	if (limit == 0)
 		return true;
-	Vtx<KW> cur = start;
+	V cur = start;
 	// explicit stack, depth <= limit <= 8: remaining-neighbour mask and dropped base per level
 	unsigned masks[8], dropped[8];
 	unsigned sp = 0;
@@ -444,12 +449,12 @@ ABB_HD bool look_ahead(Ctx& c, const Vtx<KW>& start, Dir dir, unsigned limit)
 // ------------------------------------------------------------------------------------------
 // trueBranch (Graph/ExtendPath.h:173-261), iterative; the DFS stack doubles as `visited`
 // ------------------------------------------------------------------------------------------
-template <int KW, class Ctx>
-ABB_HD bool true_branch(Ctx& c, const Vtx<KW>& u, Dir dir, unsigned base, unsigned trim_i)
+template <class V, class Ctx>
+ABB_HD bool true_branch(Ctx& c, const V& u, Dir dir, unsigned base, unsigned trim_i)
 {
 	if (trim_i == 0) // "depth >= trim" with an empty visited set
 		return true;
-	Vtx<KW> cur = u;
+	V cur = u;
 	const uint64_t hu_top = u.canon();
 	unsigned out = vtx_step(cur, c.k, c.rt, dir, base);
 	unsigned sp = 0;
@@ -546,8 +551,8 @@ ABB_HD bool true_branch(Ctx& c, const Vtx<KW>& u, Dir dir, unsigned base, unsign
 // successor (Graph/ExtendPath.h:314-362)
 // ------------------------------------------------------------------------------------------
 /** nbmask = c.neighbors(u).  Returns the result code; *vbase = base of the last true branch seen */
-template <int KW, class Ctx>
-ABB_HD ExtCode successor(Ctx& c, const Vtx<KW>& u, unsigned nbmask, Dir dir, unsigned* vbase)
+template <class V, class Ctx>
+ABB_HD ExtCode successor(Ctx& c, const V& u, unsigned nbmask, Dir dir, unsigned* vbase)
 {
 	const unsigned m = dir == FWD ? (nbmask & 15) : (nbmask >> 4);
 	// i = 0: every existing neighbour is a true branch (depth 0 >= trim 0), so the count is the degree

@@ -2,18 +2,20 @@
 //   build -t konnector (default; CityHash, -l levels, -L N=FILE, -w M/N windows, -h seed), -t counting
 //     (CountingBloomFilter<uint8_t>, the filter abyss-bloom-dbg loads with -i) and -t rolling-hash [-l LEVELS]
 //     (HashAgnosticCascadingBloom, last level serialised);
-//   union, intersect, info, compare, kmers (getKmers) on Konnector files, and info on the two BTL formats.
-// Output files and printed text are byte-compatible with the reference's.  `graph` and `trim` are not implemented (DESIGN.md
-// section 7): `graph` orders its output by a std::unordered_set.
+//   union, intersect, info, compare, kmers (getKmers), trim on Konnector files, and info on the two BTL formats.
+// Output files and printed text are byte-compatible with the reference's.  `graph` is not implemented (DESIGN.md section 7):
+// it orders its output by a std::unordered_set.
 //
 //   abyss-bloom build [-v] -k K [-b SIZE] [-h SEED] [-l LEVELS] [-L N=FILE] [-w M/N] [-t konnector|counting|rolling-hash] OUT.bloom READS...
 //   abyss-bloom union|intersect -k K OUT.bloom IN.bloom IN.bloom...
 //   abyss-bloom info [-k K] IN.bloom
 //   abyss-bloom compare -k K [-m jaccard|forbes|czekanowski] A.bloom B.bloom    (exits with status 1, as the reference does)
 //   abyss-bloom kmers -k K [-r] [--fasta|--bed|--raw] IN.bloom READS
+//   abyss-bloom trim [-v...] -k K [-q N] IN.bloom READS... > trimmed.fq
 #include "../../include/abyss_b200.h"
 #include "bloom_file.h"
 #include "reads.h"
+#include "trim.h"
 #include <getopt.h>
 #include <cmath>
 #include <iomanip>
@@ -120,10 +122,10 @@ static T parse_num(int c, const char* optarg)
 	return v;
 }
 
-/** the options of union / intersect / info / compare / kmers */
+/** the options of union / intersect / info / compare / kmers / trim */
 struct KonOpts {
 	unsigned k = 0;
-	int verbose = 0, device = 0, format = FMT_FASTA;
+	int verbose = 0, device = 0, format = FMT_FASTA, qualityThreshold = 0;
 	bool inverse = false;
 	std::string method = "jaccard";
 	uint64_t batchReads = 4000000;
@@ -138,6 +140,7 @@ static KonOpts parse_kon_opts(int argc, char** argv, const std::string& cmd)
 		case '?': usage(); break;
 		case 'k': o.k = parse_num<unsigned>(c, optarg); break;
 		case 'v': ++o.verbose; break;
+		case 'q': o.qualityThreshold = atoi(optarg); break;
 		case 'm':
 			if (cmd == "compare") {
 				o.method = optarg;
@@ -483,6 +486,80 @@ static int kmers(int argc, char** argv)
 	return EXIT_SUCCESS;
 }
 
+/** trim (bloom.cc:1292-1382): cut the read ends that are tips of the filter's de Bruijn graph; the scans run on the GPU
+ *  (abb_trim_reads), the records are written in file order */
+static int trim(int argc, char** argv)
+{
+	const KonOpts o = parse_kon_opts(argc, argv, "trim");
+	if (argc - optind < 2) {
+		std::cerr << PROGRAM ": missing arguments\n";
+		usage();
+	}
+	if (o.k < 2) { // the reference's k - 2 wraps
+		std::cerr << PROGRAM ": trim needs k >= 2\n";
+		exit(EXIT_FAILURE);
+	}
+	const std::string path = argv[optind++];
+	if (o.verbose)
+		std::cerr << "Loading bloom filter from `" << path << "'...\n";
+	KonnectorHeader h;
+	abb_filter* f = load_konnector(path, o.k, o.device, &h);
+	uint64_t pop = 0;
+	check(abb_filter_level_popcount(f, 0, &pop), "popcount");
+	if (o.verbose)
+		print_bloom_stats(h.full, pop);
+	uint64_t minBranchLen = 0;
+	if (!trim_min_branch_len(pop, h.full, &minBranchLen) || minBranchLen > 0xffffffffULL) {
+		// FPR = 1: the reference divides by log(1) = 0 and converts the infinity to size_t, which is undefined
+		std::cerr << PROGRAM ": every bit of `" << path << "' is set: there is no branch length threshold for such a filter\n";
+		exit(EXIT_FAILURE);
+	}
+	if (o.verbose >= 2)
+		std::cerr << "min length threshold for true branches (k-mers): " << minBranchLen << std::endl;
+	ReadOpts ropt;
+	ropt.chastityFilter = g_chastity;
+	ropt.trimMasked = g_trimMasked;
+	ropt.qualityOffset = g_qualityOffset;
+	ropt.qualityThreshold = o.qualityThreshold;
+	ropt.keepText = true;
+	std::vector<uint32_t> left, right;
+	std::string buf;
+	uint64_t readCount = 0;
+	for (int i = optind; i < argc; ++i) {
+		if (o.verbose)
+			std::cerr << "Reading `" << argv[i] << "'..." << std::endl;
+		host::BatchStream stream({ argv[i] }, ropt, o.batchReads, 0, false);
+		while (const ReadBatch* batch = stream.next()) {
+			left.resize(batch->size());
+			right.resize(batch->size());
+			const int rc = abb_trim_reads(f, batch->bases.data(), batch->offsets.data(), batch->size(), (unsigned)minBranchLen, left.data(), right.data());
+			if (rc != ABB_OK) {
+				std::cerr << PROGRAM ": trim: `" << argv[i] << "', batch starting at read " << readCount << ": " << abb_last_error() << "\n";
+				exit(EXIT_FAILURE);
+			}
+			for (size_t r = 0; r < batch->size(); ++r, ++readCount) {
+				const uint64_t b0 = batch->offsets[r], len = batch->offsets[r + 1] - b0;
+				// the progress line is only reached by the reads that were printed after trimming (bloom.cc:1360-1370)
+				const uint64_t i0 = batch->id_offsets[r];
+				if (append_trimmed_record(buf, batch->id_chars.data() + i0, batch->id_offsets[r + 1] - i0, batch->comment(r), batch->comment_len(r),
+				                          batch->bases.data() + b0, len, batch->qual(r), batch->qual_len(r), o.k, left[r], right[r]) &&
+				    o.verbose && (readCount + 1) % 100000 == 0)
+					std::cerr << "Processed " << (readCount + 1) << " reads" << std::endl;
+				if (buf.size() > (8u << 20)) {
+					fwrite(buf.data(), 1, buf.size(), stdout);
+					buf.clear();
+				}
+			}
+		}
+	}
+	fwrite(buf.data(), 1, buf.size(), stdout);
+	fflush(stdout);
+	if (o.verbose)
+		std::cerr << "Processed " << readCount << " reads" << std::endl;
+	abb_filter_destroy(f);
+	return EXIT_SUCCESS;
+}
+
 int main(int argc, char** argv)
 {
 	const std::string cmd = argc >= 2 ? argv[1] : "";
@@ -504,7 +581,9 @@ int main(int argc, char** argv)
 		return compare(argc, argv);
 	if (cmd == "kmers" || cmd == "getKmers")
 		return kmers(argc, argv);
-	if (cmd == "graph" || cmd == "trim") {
+	if (cmd == "trim")
+		return trim(argc, argv);
+	if (cmd == "graph") {
 		std::cerr << PROGRAM ": `" << cmd << "' is not implemented on the GPU (DESIGN.md section 7)\n";
 		usage();
 	}

@@ -37,6 +37,9 @@ struct ReadOpts {
 	int qualityThreshold = 0;
 	int internalQThreshold = 0;
 	int qualityOffset = 0; // opt::qualityOffset: 0 = the format's own (33 for FASTA / FASTQ / SAM, 64 for qseq / export)
+	// keep each record's comment and quality string as FastaReader::read returns them (for programs that write records back
+	// out: abyss-bloom trim).  Off, the reader stores neither and a ReadBatch carries ids and bases only.
+	bool keepText = false;
 };
 
 /** growable byte buffer that does not zero-fill (std::vector<char>::resize would touch every byte twice) */
@@ -62,19 +65,36 @@ struct RawBuf {
 	}
 };
 
-/** a batch of reads: concatenated bases + offsets; ids concatenated the same way (for the FASTA comments) */
+/** a batch of reads: concatenated bases + offsets; ids concatenated the same way (for the FASTA comments).  With
+ *  ReadOpts::keepText the comments and quality strings too (text_offsets has two entries per read: the comment of read i
+ *  is text_chars[text_offsets[2i], text_offsets[2i+1]), its quality string, empty for a record without one, the next range). */
 struct ReadBatch {
 	std::vector<char> bases;
 	std::vector<uint64_t> offsets{ 0 };
 	std::vector<char> id_chars;
 	std::vector<uint64_t> id_offsets{ 0 };
+	std::vector<char> text_chars;
+	std::vector<uint64_t> text_offsets{ 0 };
 	void clear()
 	{
 		bases.clear();
 		offsets.assign(1, 0);
 		id_chars.clear();
 		id_offsets.assign(1, 0);
+		text_chars.clear();
+		text_offsets.assign(1, 0);
 	}
+	void add_text(const std::string& comment, const std::string& qual)
+	{
+		text_chars.insert(text_chars.end(), comment.begin(), comment.end());
+		text_offsets.push_back(text_chars.size());
+		text_chars.insert(text_chars.end(), qual.begin(), qual.end());
+		text_offsets.push_back(text_chars.size());
+	}
+	const char* comment(size_t i) const { return text_chars.data() + text_offsets[2 * i]; }
+	size_t comment_len(size_t i) const { return (size_t)(text_offsets[2 * i + 1] - text_offsets[2 * i]); }
+	const char* qual(size_t i) const { return text_chars.data() + text_offsets[2 * i + 1]; }
+	size_t qual_len(size_t i) const { return (size_t)(text_offsets[2 * i + 2] - text_offsets[2 * i + 1]); }
 	size_t size() const { return offsets.size() - 1; }
 	void add(const std::string& id, const std::string& seq)
 	{
@@ -166,6 +186,9 @@ class SeqReader {
 
 	/** the comment (rest of the header line after the id) of the record the last next() returned */
 	const std::string& last_comment() const { return m_comment; }
+	/** its quality string after the reader's trimming, empty when the record has none; kept only with ReadOpts::keepText or a
+	 *  quality threshold */
+	const std::string& last_quality() const { return m_q; }
 
 	/** next record; false at end of file */
 	bool next(std::string& id, std::string& seq)
@@ -210,7 +233,7 @@ class SeqReader {
 			}
 			line(l, n);
 			seq.assign(l, n);
-			const bool needq = m_opt.qualityThreshold > 0 || m_opt.internalQThreshold > 0;
+			const bool needq = m_opt.qualityThreshold > 0 || m_opt.internalQThreshold > 0 || m_opt.keepText;
 			size_t qlen = 0;
 			bool haveq = false;
 			if (type == '>') {
@@ -656,6 +679,12 @@ class BatchStream {
 			o[r] = so[r] + d;
 			io[r] = sio[r] + di;
 		}
+		if (m_opt.keepText) {
+			const uint64_t t0 = b.text_offsets[2 * r0], t1 = b.text_offsets[2 * (r0 + n)], dt = m_out.text_chars.size() - t0;
+			m_out.text_chars.insert(m_out.text_chars.end(), b.text_chars.begin() + t0, b.text_chars.begin() + t1);
+			for (size_t j = 2 * r0 + 1; j <= 2 * (r0 + n); ++j)
+				m_out.text_offsets.push_back(b.text_offsets[j] + dt);
+		}
 	}
 	/** hand a parsed piece to next() */
 	void publish(uint64_t seq, std::unique_ptr<ReadBatch> b)
@@ -705,13 +734,19 @@ class BatchStream {
 			std::string id, seq;
 			if (pc.view) {
 				SeqReader in(pc.view, pc.view_len, pc.path, m_opt, pc.view_off, pc.map->base);
-				while (in.next(id, seq))
+				while (in.next(id, seq)) {
 					b->add(id, seq);
+					if (m_opt.keepText)
+						b->add_text(in.last_comment(), in.last_quality());
+				}
 				pc.map.reset(); // the last piece of a file unmaps it
 			} else {
 				SeqReader in(std::move(pc.data), pc.path, m_opt, pc.first_line);
-				while (in.next(id, seq))
+				while (in.next(id, seq)) {
 					b->add(id, seq);
+					if (m_opt.keepText)
+						b->add_text(in.last_comment(), in.last_quality());
+				}
 				std::lock_guard<std::mutex> l(m_mu);
 				m_freeBufs.push_back(in.release());
 			}

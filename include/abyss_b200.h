@@ -95,6 +95,22 @@ int abb_filter_compare(abb_filter* a, abb_filter* b, uint64_t counts[4]);
 /* set bits of one level (-1 = the last) of a bit filter (ABB_BIT, ABB_CASCADING, ABB_KONNECTOR) */
 int abb_filter_level_popcount(abb_filter* f, int level, uint64_t* n);
 
+/* `abyss-bloom trim` (Bloom/bloom.cc:1233-1382): for every read, the number of bases to cut from its left end and from its
+ * right end because they are a tip of the Bloom filter de Bruijn graph (Konnector/DBGBloom.h: vertices are k-mers as given,
+ * not up to reverse complement; a k-mer is a vertex when its canonical form is in the filter; out- and in-neighbours in the
+ * order A, C, G, T).  left[r] is calcLeftTrim (bloom.cc:1236-1290) of read r and right[r] calcLeftTrim of its reverse
+ * complement: the windows are scanned with KmerIterator's rules (those holding a non-ACGT character are skipped), k-mers not
+ * in the filter are skipped, each k-mer in the filter is judged by successor() to either side (Graph/ExtendPath.h:314-362,
+ * trim = min_branch_len, fpTrim = 5), the first one stops the scan unless it is a tip, a later one stops it at a fork, and
+ * stopping at window p gives p == 0 ? 0 : k + p - 1.  A scan that runs off the end gives k - 2, as the reference's does
+ * (its iterator's pos() is SIZE_MAX then); a read shorter than k gives 0 and 0 (trim() echoes it).  The caller prints bases
+ * [left, len - 1 - right] when that range is not empty (bloom.cc:1353-1367).  A filter of several levels is probed at its
+ * last level, as abb_contains_reads does.  min_branch_len is ceil(log(0.0001) / log(popcount / size)) in the reference
+ * (bloom.cc:1324-1327).  bases / offsets as for abb_insert_reads.  ABB_ESTATE for a filter that is not a Konnector filter,
+ * and when the branch search of a read outgrows its scratch memory (the message names the read; no length is guessed). */
+int abb_trim_reads(abb_filter* f, const char* bases, const uint64_t* offsets, uint64_t n_reads, unsigned min_branch_len, uint32_t* left,
+                   uint32_t* right);
+
 /* ---- pass 1: loadSeq / loadFile (BloomDBG/BloomIO.h:32-41,50-94) --------------------------
  * Hash every k-mer of every read (RollingHashIterator semantics: upper-cased, windows touching a
  * non-ACGT base skipped) and insert it, with results IDENTICAL to inserting read by read, k-mer

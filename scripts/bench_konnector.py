@@ -5,8 +5,11 @@ Workload `m1_k64`: 1 M x 150 bp reads of a 5 Mbp genome (abyss_b200.synth seed 7
 Reports, as one JSON line:
   build_kmers_per_s   abb_insert_reads on the whole batch (reads already in host memory), best of --steps
   query_kmers_per_s   abb_contains_reads (the kmers command's query) on the same reads against the built filter
-  cli_build_s / cli_kmers_s   wall time of `abyss-bloom build` and `abyss-bloom kmers --raw` on the FASTQ (parse + GPU + file I/O)
-  ref_build_s / ref_kmers_s   the same commands of the reference (oracle/_ref/abyss-bloom-ref, -j8 for build) when built
+  trim_reads_per_s, trim_ms   abb_trim_reads on the same reads against the built filter (minBranchLen from its population):
+                      host wall time of the call (copies included, it ends in a synchronise) and CUDA events on the library's
+                      stream around it
+  cli_build_s / cli_kmers_s / cli_trim_s   wall time of `abyss-bloom build`, `kmers --raw` and `trim` on the FASTQ (parse + GPU + file I/O)
+  ref_build_s / ref_kmers_s / ref_trim_s   the same commands of the reference (oracle/_ref/abyss-bloom-ref, -j8 for build) when built
   gpu, power_limit    the card and its power limit, queried in the same run
 Everything it writes goes to a temporary directory.
 
@@ -15,6 +18,7 @@ Everything it writes goes to a temporary directory.
 import argparse
 import ctypes as C
 import json
+import math
 import os
 import subprocess
 import sys
@@ -58,7 +62,8 @@ def main():
     lib = capi.load()
     res = {"workload": "m1_k64: 1 M x 150 bp, k=64, -b1G -l2", "kmer_windows": n_kmers}
     bits = BYTES * 8 // LEVELS
-    best_ins, best_q = float("inf"), float("inf")
+    best_ins, best_q, best_t, best_t_ev = float("inf"), float("inf"), float("inf"), float("inf")
+    import torch
     for _ in range(a.steps):
         f = capi.Filter.konnector(bits, K, LEVELS)
         t0 = time.perf_counter()
@@ -74,9 +79,22 @@ def main():
         capi.check(lib.abb_contains_reads(q.handle, capi._ptr(bases), capi._ptr(offs), rs.n, capi._ptr(flag), capi._ptr(valid), n_kmers,
                                           C.byref(n)))
         best_q = min(best_q, time.perf_counter() - t0)
+        mbl = math.ceil(math.log(0.0001) / math.log(q.level_popcount() / bits))
+        stream = torch.cuda.ExternalStream(q.stream())
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record(stream)
+        t0 = time.perf_counter()
+        q.trim_reads((bases, offs), mbl)
+        best_t = min(best_t, time.perf_counter() - t0)
+        e1.record(stream)
+        e1.synchronize()
+        best_t_ev = min(best_t_ev, e0.elapsed_time(e1))
         q.close()
     res["build_kmers_per_s"] = n_kmers / best_ins
     res["query_kmers_per_s"] = n_kmers / best_q
+    res["trim_min_branch_len"] = mbl
+    res["trim_reads_per_s"] = rs.n / best_t
+    res["trim_ms"] = best_t_ev
     exe = os.path.join(ROOT, "abyss_b200", "lib", "abyss-bloom")
     ref = os.path.join(ROOT, "oracle", "_ref", "abyss-bloom-ref")
     with tempfile.TemporaryDirectory() as d:
@@ -85,9 +103,11 @@ def main():
         dn = subprocess.DEVNULL
         res["cli_build_s"] = timed([exe, "build", f"-k{K}", "-b1G", f"-l{LEVELS}", os.path.join(d, "g.bloom"), fq], stderr=dn)
         res["cli_kmers_s"] = timed([exe, "kmers", f"-k{K}", "--raw", os.path.join(d, "g.bloom"), fq], stdout=dn)
+        res["cli_trim_s"] = timed([exe, "trim", f"-k{K}", os.path.join(d, "g.bloom"), fq], stdout=dn)
         if os.path.exists(ref) and not a.no_ref:
             res["ref_build_s"] = timed([ref, "build", f"-k{K}", "-b1G", f"-l{LEVELS}", "-j8", os.path.join(d, "r.bloom"), fq], stderr=dn)
             res["ref_kmers_s"] = timed([ref, "kmers", f"-k{K}", "--raw", os.path.join(d, "r.bloom"), fq], stdout=dn)
+            res["ref_trim_s"] = timed([ref, "trim", f"-k{K}", os.path.join(d, "r.bloom"), fq], stdout=dn)
         else:
             res["ref"] = "oracle/_ref/abyss-bloom-ref not built: no CPU figures"
     res["gpu"], res["power_limit"] = card()

@@ -397,10 +397,7 @@ int launch_hash_segments(unsigned k, const uint8_t* d_care, const uint8_t* d_bas
 {
 	if (n_segs == 0)
 		return ABB_OK;
-	int sms = 132, dev = 0;
-	cudaGetDevice(&dev);
-	cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-	const unsigned grid = (unsigned)std::min<uint64_t>((n_segs + kHashWarps - 1) / kHashWarps, (uint64_t)sms * 32);
+	const unsigned grid = (unsigned)std::min<uint64_t>((n_segs + kHashWarps - 1) / kHashWarps, (uint64_t)sm_count() * 32);
 	if (d_care)
 		k_hash_segments_masked<<<grid, kHashWarps * 32, 0, stream>>>(d_bases, d_seg_beg, d_seg_len, d_seg_slot, n_segs, k, d_care,
 		                                                             d_h0, d_valid);

@@ -161,7 +161,7 @@ struct WarpCtx {
 			off = atomicAdd(arena_top, bytes);
 		off = __shfl_sync(0xffffffffu, off, 0);
 		if (off + bytes > arena_size) {
-			fail(3);
+			fail(WALK_FAIL_ARENA);
 			return nullptr;
 		}
 		uint8_t* p = arena + off;
@@ -589,7 +589,7 @@ k_extend(const uint8_t* __restrict__ bases, const uint64_t* __restrict__ offs, c
 	DevEmit emit = { recs, nrecs, rec_cap, gwarp, 0 };
 	const bool ok = walk_read<KW>(c, bases + beg, L, emit);
 	if (c.lane == 0)
-		status[gwarp] = ok ? 0u : (c.fail_ ? c.fail_ : 1u);
+		status[gwarp] = ok ? 0u : (c.fail_ ? c.fail_ : walk_fail_bit(WALK_FAIL_NO_CODE));
 }
 
 
@@ -1225,8 +1225,6 @@ struct abb_assembler {
 	DevBuf<TileRec> tile_export;
 	DevBuf<uint8_t> stage_bases, rep_flag;
 	DevBuf<uint64_t> stage_hashes;
-	uint64_t st_markers = 0, st_tiles = 0, st_fallbacks = 0;
-	float ms_tiles = 0, ms_walk = 0, ms_stage = 0, ms_repeat = 0, ms_total = 0, ms_cand = 0;
 
 	// speculation control
 	unsigned spec_target = 512;
@@ -1235,27 +1233,19 @@ struct abb_assembler {
 	std::vector<char> out_seqs;
 	std::vector<uint8_t> out_codes;
 	std::vector<abb_trace_row> out_trace; // one row per contig handed to outputContig (params.reserved & 1)
-	// statistics
-	uint64_t st_iterations = 0, st_speculated = 0, st_wasted = 0, st_launches = 0, st_candidates = 0, st_contigs_tried = 0;
-	float ms_classify = 0, ms_visited = 0, ms_extend = 0, ms_replay = 0;
-	Event ev[2], ev2[2];
+	abb_assembly_stats st = {};
+	// launch geometry, fixed by the device and k of this assembler: SMs, the CTAs of k_make_tiles<kw> that are resident at
+	// once, and the largest grid k_replay_all can be launched with cooperatively
+	unsigned sms = 0, tile_ctas = 0, replay_grid = 0;
+	Event ev[2], ev2[2]; // a phase (ms_classify, ms_tiles, ms_visited, ms_extend, ms_replay) / a stretch inside ms_extend
+
+	unsigned world() const { return comm ? (unsigned)abb_comm_world(comm) : 1u; }
+	unsigned rank() const { return comm ? (unsigned)abb_comm_rank(comm) : 0u; }
+	StreamTimer time_phase(float* acc) { return StreamTimer(ev[0], ev[1], stream, acc); }
+	StreamTimer time_inner(float* acc) { return StreamTimer(ev2[0], ev2[1], stream, acc); }
 };
 
 namespace {
-
-struct PhaseTimer { // CUDA-event time of a phase on the assembler stream
-	abb_assembler* a;
-	float* acc;
-	PhaseTimer(abb_assembler* a_, float* acc_) : a(a_), acc(acc_) { cudaEventRecord(a->ev[0], a->stream); }
-	void stop()
-	{
-		cudaEventRecord(a->ev[1], a->stream);
-		cudaEventSynchronize(a->ev[1]);
-		float ms = 0;
-		cudaEventElapsedTime(&ms, a->ev[0], a->ev[1]);
-		*acc += ms;
-	}
-};
 
 constexpr unsigned kMaxSpec = 1024;
 constexpr unsigned kMinSpec = 256;   // with tiles a round costs about the same latency for 64 or 1024 walkers, and wasted walks are cheap
@@ -1336,25 +1326,31 @@ int h2d(DevBuf<T>& d, const std::vector<T>& h, cudaStream_t s)
 	return ABB_OK;
 }
 
-/** rank r holds `mine` = n_r bytes (n_r = its slice of n_total split as [r*n/w, (r+1)*n/w)); afterwards `all` holds the
- *  n_total bytes of every rank's slice in rank order.  One ncclAllGather over slices padded to the longest. */
+/** the part [lo, up) of n items that rank r of `world` works on; what is sharded and all-gathered is split like this */
+struct Slice {
+	uint64_t lo, up;
+};
+Slice slice_of(uint64_t n, unsigned r, unsigned world) { return { (uint64_t)r * n / world, (uint64_t)(r + 1) * n / world }; }
+
+/** this rank holds `mine` = the bytes of its slice of n_total; afterwards `all` holds the n_total bytes of every rank's
+ *  slice in rank order.  One ncclAllGather over slices padded to the longest. */
 int allgather_slices(abb_assembler* a, const uint8_t* mine, uint64_t n_total, uint8_t* all)
 {
-	const unsigned world = (unsigned)abb_comm_world(a->comm), rank = (unsigned)abb_comm_rank(a->comm);
+	const unsigned world = a->world(), rank = a->rank();
 	cudaStream_t st = a->stream;
 	uint64_t mx = 0;
 	for (unsigned r = 0; r < world; ++r)
-		mx = std::max<uint64_t>(mx, (r + 1) * n_total / world - r * n_total / world);
+		mx = std::max<uint64_t>(mx, slice_of(n_total, r, world).up - slice_of(n_total, r, world).lo);
 	mx = (mx + 15) & ~15ULL;
 	ABB_CHECK(a->gather.reserve(world * mx));
-	const uint64_t lo = rank * n_total / world, up = (rank + 1) * n_total / world;
-	if (up > lo)
-		ABB_CUDA(cudaMemcpyAsync(a->gather.p + rank * mx, mine, up - lo, cudaMemcpyDeviceToDevice, st));
+	const Slice my = slice_of(n_total, rank, world);
+	if (my.up > my.lo)
+		ABB_CUDA(cudaMemcpyAsync(a->gather.p + rank * mx, mine, my.up - my.lo, cudaMemcpyDeviceToDevice, st));
 	ABB_CHECK(abb_comm_allgather_bytes(a->comm, a->gather.p, mx, st));
 	for (unsigned r = 0; r < world; ++r) {
-		const uint64_t l = r * n_total / world, u = (r + 1) * n_total / world;
-		if (u > l)
-			ABB_CUDA(cudaMemcpyAsync(all + l, a->gather.p + r * mx, u - l, cudaMemcpyDeviceToDevice, st));
+		const Slice sl = slice_of(n_total, r, world);
+		if (sl.up > sl.lo)
+			ABB_CUDA(cudaMemcpyAsync(all + sl.lo, a->gather.p + r * mx, sl.up - sl.lo, cudaMemcpyDeviceToDevice, st));
 	}
 	return ABB_OK;
 }
@@ -1422,7 +1418,7 @@ int ensure_tile_store(abb_assembler* a)
 int exchange_tiles(abb_assembler* a, unsigned n0, unsigned n1, unsigned long long p0, unsigned long long p1)
 {
 	cudaStream_t st = a->stream;
-	const unsigned world = (unsigned)abb_comm_world(a->comm), rank = (unsigned)abb_comm_rank(a->comm);
+	const unsigned world = a->world(), rank = a->rank();
 	// 1. how much does everybody have?
 	ABB_CHECK(a->gather.reserve(world * 16 + 16));
 	unsigned long long mine[2] = { n1 - n0, p1 - p0 };
@@ -1463,7 +1459,7 @@ int exchange_tiles(abb_assembler* a, unsigned n0, unsigned n1, unsigned long lon
 	ABB_CUDA(cudaMemcpyAsync(a->d_tile_n.p, &nt32, sizeof nt32, cudaMemcpyHostToDevice, st));
 	ABB_CUDA(cudaMemcpyAsync(a->d_tile_pool_top.p, &pt, sizeof pt, cudaMemcpyHostToDevice, st));
 	ABB_CUDA(cudaStreamSynchronize(st));
-	a->st_launches += 2 + world;
+	a->st.launches += 2 + world;
 	return ABB_OK;
 }
 
@@ -1472,16 +1468,16 @@ int produce_tiles(abb_assembler* a, uint64_t n_reads, uint64_t n_slots)
 {
 	if (!a->tiles_on || n_slots == 0)
 		return ABB_OK;
-	PhaseTimer tt(a, &a->ms_tiles);
+	StreamTimer tt = a->time_phase(&a->st.ms_tiles);
 	ABB_CHECK(ensure_tile_store(a));
 	abb_filter* f = a->solid;
 	cudaStream_t st = a->stream;
 	const WalkCfg w = walk_cfg(a);
-	const unsigned world = a->comm ? (unsigned)abb_comm_world(a->comm) : 1u, rank = a->comm ? (unsigned)abb_comm_rank(a->comm) : 0u;
+	const unsigned world = a->world(), rank = a->rank();
 	const unsigned out_cap = (unsigned)std::min<uint64_t>(n_slots / (kMarkerMask + 1) * 2 + 4096, a->marker_set_mask / 2 + 1);
 	ABB_CHECK(a->new_markers.reserve(out_cap));
 	ABB_CUDA(cudaMemsetAsync(a->d_tile_n.p + 1, 0, 2 * sizeof(unsigned), st));
-	k_find_markers<<<sm_count() * 16, 256, 0, st>>>(a->h0.p, a->valid.p, a->slot_offs.p, n_reads, n_slots, w, f->cfg, a->d_marker_set.p,
+	k_find_markers<<<a->sms * 16, 256, 0, st>>>(a->h0.p, a->valid.p, a->slot_offs.p, n_reads, n_slots, w, f->cfg, a->d_marker_set.p,
 	                                         a->marker_set_mask, a->new_markers.p, a->d_tile_n.p + 2, out_cap, world, rank);
 	ABB_CUDA(cudaGetLastError());
 	unsigned nm = 0, n0 = 0;
@@ -1492,22 +1488,12 @@ int produce_tiles(abb_assembler* a, uint64_t n_reads, uint64_t n_slots)
 	ABB_CUDA(cudaStreamSynchronize(st));
 	nm = std::min(nm, out_cap);
 	n0 = std::min(n0, a->tile_cap);
-	a->st_launches += 1;
-	if (nm == 0 && world == 1) {
-		tt.stop();
+	a->st.launches += 1;
+	if (nm == 0 && world == 1)
 		return ABB_OK;
-	}
 	if (nm) {
-		int sms = 132;
-		cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, f->device);
 		// persistent warps pulling (marker, orientation, direction) items from a counter: as many CTAs as fit
-		static int tiles_per_sm = 0;
-		if (tiles_per_sm == 0) {
-			int n = 0;
-			ABB_DISPATCH_KW(a->kw, (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_make_tiles<KW>, kWalkWarps * 32, 0)));
-			tiles_per_sm = std::max(1, n);
-		}
-		const unsigned grid = (unsigned)std::min<uint64_t>(blocks_for((uint64_t)nm * 4, kWalkWarps), (uint64_t)sms * tiles_per_sm);
+		const unsigned grid = std::min(blocks_for((uint64_t)nm * 4, kWalkWarps), a->tile_ctas);
 		const unsigned warps = grid * kWalkWarps;
 		ABB_CHECK(ensure_scratch(a, warps));
 		ABB_CHECK(a->stage_bases.reserve((size_t)warps * kTileCap));
@@ -1518,7 +1504,7 @@ int produce_tiles(abb_assembler* a, uint64_t n_reads, uint64_t n_slots)
 		                                                                          a->d_tile_n.p + 1, w, f->cfg, a->frames.p, a->look.p,
 		                                                                          a->stage_bases.p, a->stage_hashes.p, ts)));
 		ABB_CUDA(cudaGetLastError());
-		a->st_launches += 1;
+		a->st.launches += 1;
 	}
 	unsigned nt = 0;
 	unsigned long long p1 = 0;
@@ -1527,18 +1513,17 @@ int produce_tiles(abb_assembler* a, uint64_t n_reads, uint64_t n_slots)
 	ABB_CUDA(cudaStreamSynchronize(st));
 	nt = std::min(nt, a->tile_cap);
 	p1 = std::min(p1, a->tile_pool_size);
-	a->st_markers += nm;
-	a->st_tiles = nt;
+	a->st.markers += nm;
+	a->st.tiles = nt;
 	if (world > 1) {
 		ABB_CHECK(exchange_tiles(a, n0, nt, p0, p1));
 		ABB_CUDA(cudaMemcpyAsync(&nt, a->d_tile_n.p, sizeof nt, cudaMemcpyDeviceToHost, st));
 		ABB_CUDA(cudaStreamSynchronize(st));
-		a->st_tiles = nt;
+		a->st.tiles = nt;
 	}
-	k_link_tiles<<<sm_count() * 8, 256, 0, st>>>(a->d_tiles.p, (unsigned)a->st_tiles, a->d_tile_tab.p, a->tile_tab_mask);
+	k_link_tiles<<<a->sms * 8, 256, 0, st>>>(a->d_tiles.p, (unsigned)a->st.tiles, a->d_tile_tab.p, a->tile_tab_mask);
 	ABB_CUDA(cudaGetLastError());
-	a->st_launches += 1;
-	tt.stop();
+	a->st.launches += 1;
 	return ABB_OK;
 }
 
@@ -1565,29 +1550,24 @@ int run_extend(abb_assembler* a, unsigned n_spec, bool use_tiles, bool keep_aren
 		ABB_CUDA(cudaMemsetAsync(a->d_nrecs.p, 0, sizeof(unsigned), st));
 		const WalkCfg w = walk_cfg(a);
 		const TileView tv = tile_view(a, use_tiles);
-		cudaEventRecord(a->ev2[0], st);
+		StreamTimer tw = a->time_inner(&a->st.ms_walk); // read where this turn of the loop ends, after the synchronise below
 		ABB_DISPATCH_KW(a->kw, (k_extend<KW><<<blocks_for(n_spec, kWalkWarps), kWalkWarps * 32, 0, st>>>(
 		                           a->cur_bases, a->cur_offs, a->spec.p, n_spec, w, f->cfg, a->frames.p, a->look.p, a->d_arena.p, a->arena_size,
 		                           a->d_arena_top.p, a->recs.p, a->d_nrecs.p, rec_cap, a->status.p, tv)));
 		ABB_CUDA(cudaGetLastError());
-		cudaEventRecord(a->ev2[1], st);
-		++a->st_launches;
+		tw.end();
+		++a->st.launches;
 		unsigned nrecs = 0;
 		ABB_CUDA(cudaMemcpyAsync(&nrecs, a->d_nrecs.p, sizeof nrecs, cudaMemcpyDeviceToHost, st));
 		ABB_CUDA(cudaMemcpyAsync(status.data(), a->status.p, n_spec * sizeof(unsigned), cudaMemcpyDeviceToHost, st));
 		ABB_CUDA(cudaStreamSynchronize(st));
-		{
-			float ms = 0;
-			cudaEventElapsedTime(&ms, a->ev2[0], a->ev2[1]);
-			a->ms_walk += ms;
-		}
 		if (nrecs > rec_cap) { // record buffer too small: rerun with room for everything
 			rec_cap = nrecs + nrecs / 4 + 16;
 			continue;
 		}
 		bool arena_fail = false;
 		for (unsigned i = 0; i < n_spec; ++i)
-			arena_fail |= (status[i] & (1u << 3)) != 0;
+			arena_fail |= (status[i] & walk_fail_bit(WALK_FAIL_ARENA)) != 0;
 		if (arena_fail && !keep_arena) {
 			// out of unitig scratch: grow the arena (free memory permitting) and rerun
 			size_t free_b = 0, total_b = 0;
@@ -1668,318 +1648,346 @@ int stage_contigs(abb_assembler* a, const std::vector<ContigRec>& recs, const Ro
 		ABB_CHECK(h2d(a->seg_len, seg_len, st));
 		ABB_CHECK(h2d(a->seg_beg, seg_beg, st));
 		ABB_CHECK(h2d(a->seg_slot, seg_slot, st));
-		cudaEventRecord(a->ev2[0], st);
-		k_gather<<<std::min<unsigned>(ns, sm_count() * 16), 256, 0, st>>>(a->recs_sorted.p, a->seg_contig.p, a->seg_beg.p, a->seg_len.p, ns, a->coffs.p,
+		StreamTimer ts = a->time_inner(&a->st.ms_stage);
+		k_gather<<<std::min<unsigned>(ns, a->sms * 16), 256, 0, st>>>(a->recs_sorted.p, a->seg_contig.p, a->seg_beg.p, a->seg_len.p, ns, a->coffs.p,
 		                                                          a->cseq.p, f->k, a->rt);
 		ABB_CUDA(cudaGetLastError());
 		ABB_CHECK(launch_hash_segments(f->k, f->d_care.p, a->cseq.p, a->seg_beg.p, a->seg_len.p, a->seg_slot.p, ns, a->ch0.p, a->cvalid.p, st));
-		cudaEventRecord(a->ev2[1], st);
-		cudaEventSynchronize(a->ev2[1]);
-		float ms = 0;
-		cudaEventElapsedTime(&ms, a->ev2[0], a->ev2[1]);
-		a->ms_stage += ms;
-		a->st_launches += 2;
+		a->st.launches += 2;
 	}
 	return ABB_OK;
 }
 
-/** one speculation round over candidates starting at *cursor; appends accepted contigs */
-int speculate_round(abb_assembler* a, const std::vector<unsigned>& cand, size_t* cursor, uint64_t n_reads)
+/** one speculation round: what each phase below leaves for the next */
+struct Round {
+	std::vector<unsigned> spec; // the speculated reads (indices into the batch) in file order; a->spec holds them on the device
+	unsigned n_spec = 0;        // how many were speculated
+	unsigned n_ok = 0;          // reads [0, n_ok) of spec were walked to the end; the rest go back to the queue
+	std::vector<unsigned> redo; // indices into spec of the reads to walk again vertex by vertex
+	std::vector<ContigRec> recs;
+	RoundLayout L;
+	// what the replay decided
+	std::vector<uint8_t> rcode, caccept; // per read its code, per unitig whether it was printed
+	std::vector<unsigned> ccov;
+	std::vector<uint64_t> hoff; // where each printed unitig lies in `seqs`
+	std::vector<char> seqs;
+};
+
+/** K3b over chunks of the candidates from *cursor on: the covered ones are final, the first spec_target uncovered ones
+ *  are speculated; *cursor moves past what was looked at */
+int scan_uncovered(abb_assembler* a, const std::vector<unsigned>& cand, size_t* cursor, Round& r)
 {
 	abb_filter* f = a->solid;
 	cudaStream_t st = a->stream;
 	const size_t ncand = cand.size();
-	// ---- K3b over a chunk of candidates; pick the first spec_target uncovered ones
-	std::vector<unsigned> spec;
 	size_t pos = *cursor;
 	size_t chunk = std::max<size_t>(a->spec_target, 1024);
-	PhaseTimer tv(a, &a->ms_visited);
-	while (pos < ncand && spec.size() < a->spec_target) {
+	StreamTimer tv = a->time_phase(&a->st.ms_visited);
+	while (pos < ncand && r.spec.size() < a->spec_target) {
 		const unsigned n = (unsigned)std::min(chunk, ncand - pos);
 		ABB_CHECK(a->vis.reserve(n));
-		{
-			// pure per candidate against the CURRENT assembled filter (identical on every rank: the replay is replicated)
-			const unsigned world = a->comm ? (unsigned)abb_comm_world(a->comm) : 1u, rank = a->comm ? (unsigned)abb_comm_rank(a->comm) : 0u;
-			const unsigned vlo = (unsigned)((uint64_t)rank * n / world), vup = (unsigned)((uint64_t)(rank + 1) * n / world);
-			if (vup > vlo)
-				k_visited<<<blocks_for((uint64_t)(vup - vlo) * 32, 256), 256, 0, st>>>(a->cand.p, (unsigned)pos + vlo, vup - vlo, a->slot_offs.p, a->h0.p,
-				                                                                      f->cfg, a->assembled->d_data.p, a->vis.p + vlo);
-			ABB_CUDA(cudaGetLastError());
-			++a->st_launches;
-			if (world > 1)
-				ABB_CHECK(allgather_slices(a, a->vis.p + vlo, n, a->vis.p));
-		}
+		// pure per candidate against the CURRENT assembled filter (identical on every rank: the replay is replicated)
+		const Slice my = slice_of(n, a->rank(), a->world());
+		const unsigned vlo = (unsigned)my.lo, vup = (unsigned)my.up;
+		if (vup > vlo)
+			k_visited<<<blocks_for((uint64_t)(vup - vlo) * 32, 256), 256, 0, st>>>(a->cand.p, (unsigned)pos + vlo, vup - vlo, a->slot_offs.p, a->h0.p,
+			                                                                      f->cfg, a->assembled->d_data.p, a->vis.p + vlo);
+		ABB_CUDA(cudaGetLastError());
+		++a->st.launches;
+		if (a->world() > 1)
+			ABB_CHECK(allgather_slices(a, a->vis.p + vlo, n, a->vis.p));
 		std::vector<uint8_t> vis(n);
 		ABB_CUDA(cudaMemcpyAsync(vis.data(), a->vis.p, n, cudaMemcpyDeviceToHost, st));
 		ABB_CUDA(cudaStreamSynchronize(st));
 		size_t i = 0;
-		for (; i < n && spec.size() < a->spec_target; ++i) {
+		for (; i < n && r.spec.size() < a->spec_target; ++i) {
 			if (vis[i]) {
 				a->out_codes[cand[pos + i]] = RC_ALL_KMERS_VISITED;
 				++a->counters.visited_reads;
 			} else
-				spec.push_back(cand[pos + i]);
+				r.spec.push_back(cand[pos + i]);
 		}
 		pos += i;
 		chunk = std::min<size_t>(chunk * 4, 1u << 22);
 	}
 	*cursor = pos;
-	tv.stop();
-	if (spec.empty())
-		return ABB_OK;
-	++a->st_iterations;
-	a->st_speculated += spec.size();
+	r.n_spec = r.n_ok = (unsigned)r.spec.size();
+	return ABB_OK;
+}
 
-	// ---- K4: extend all speculated reads (tiles on), then the exact vertex-by-vertex fallback for
-	// reads whose tiled walk cycled or produced a path with a repeated vertex
-	const unsigned n_spec = (unsigned)spec.size();
-	std::vector<ContigRec> recs;
+/** K4 with tiles over all speculated reads; reads whose tile chain cycled are to be redone, the first read that ran out
+ *  of scratch ends the round (n_ok) */
+int extend_tiled(abb_assembler* a, Round& r)
+{
 	std::vector<unsigned> status;
-	RoundLayout L;
-	unsigned n_ok = n_spec;
-	{
-		PhaseTimer te(a, &a->ms_extend);
-		ABB_CHECK(h2d(a->spec, spec, st));
-		ABB_CHECK(run_extend(a, n_spec, true, false, recs, status));
-		std::vector<unsigned> redo; // indices into spec
-		for (unsigned i = 0; i < n_spec; ++i) {
-			if (status[i] & (1u << 4)) { // tile chain cycled
-				redo.push_back(i);
-				status[i] = 0;
-			}
+	ABB_CHECK(h2d(a->spec, r.spec, a->stream));
+	ABB_CHECK(run_extend(a, r.n_spec, true, false, r.recs, status));
+	for (unsigned i = 0; i < r.n_spec; ++i) {
+		if (status[i] & walk_fail_bit(WALK_FAIL_TILE_CYCLE)) {
+			r.redo.push_back(i);
+			status[i] = 0;
 		}
-		for (unsigned i = 0; i < n_spec; ++i)
-			if (status[i] != 0) {
-				n_ok = i;
-				break;
-			}
-		if (n_ok == 0) {
-			if (status[0] & ((1u << 1) | (1u << 2)))
-				set_error("graph traversal exceeded the per-warp scratch bounds (lookAhead %u / trueBranch %u frames)", kLookCap, kFrameCap);
-			else
-				set_error("unitig scratch arena exhausted at %llu bytes", a->arena_size);
-			return ABB_ENOMEM;
-		}
-		// repeat check on everything that was produced with tiles
-		if (a->tiles_on && a->d_tile_tab.p) {
-			std::vector<ContigRec> keep;
-			for (auto& r : recs)
-				if (r.spec < n_ok && std::find(redo.begin(), redo.end(), r.spec) == redo.end())
-					keep.push_back(r);
-			recs.swap(keep);
-			layout_records(recs, n_ok, f->k, L);
-			ABB_CHECK(stage_contigs(a, recs, L));
-			const unsigned nc = (unsigned)recs.size();
-			if (nc) {
-				std::vector<uint64_t> tab_off(nc + 1, 0);
-				for (unsigned c = 0; c < nc; ++c)
-					tab_off[c + 1] = tab_off[c] + 2 * (L.cslot[c + 1] - L.cslot[c]) + 8;
-				const uint64_t tab = tab_off[nc];
-				ABB_CHECK(h2d(a->rep_off, tab_off, st));
-				ABB_CHECK(a->rep_tab.reserve(tab));
-				ABB_CHECK(a->rep_flag.reserve(nc));
-				cudaEventRecord(a->ev2[0], st);
-				ABB_CUDA(cudaMemsetAsync(a->rep_tab.p, 0, tab * sizeof(unsigned long long), st));
-				ABB_CUDA(cudaMemsetAsync(a->rep_flag.p, 0, nc, st));
-				k_repeat_check<<<sm_count() * 8, 256, 0, st>>>(a->recs_sorted.p, nc, a->cslot.p, a->ch0.p, a->rep_tab.p, a->rep_off.p, a->rep_flag.p);
-				ABB_CUDA(cudaGetLastError());
-				cudaEventRecord(a->ev2[1], st);
-				++a->st_launches;
-				std::vector<uint8_t> flag(nc);
-				ABB_CUDA(cudaMemcpyAsync(flag.data(), a->rep_flag.p, nc, cudaMemcpyDeviceToHost, st));
-				ABB_CUDA(cudaStreamSynchronize(st));
-				{
-					float ms = 0;
-					cudaEventElapsedTime(&ms, a->ev2[0], a->ev2[1]);
-					a->ms_repeat += ms;
-				}
-				for (unsigned c = 0; c < nc; ++c)
-					if (flag[c] && (redo.empty() || redo.back() != recs[c].spec) &&
-					    std::find(redo.begin(), redo.end(), recs[c].spec) == redo.end())
-						redo.push_back(recs[c].spec);
-			}
-		}
-		redo.erase(std::remove_if(redo.begin(), redo.end(), [&](unsigned i) { return i >= n_ok; }), redo.end());
-		if (!redo.empty()) {
-			std::sort(redo.begin(), redo.end());
-			a->st_fallbacks += redo.size();
-			std::vector<unsigned> sub(redo.size());
-			for (size_t i = 0; i < redo.size(); ++i)
-				sub[i] = spec[redo[i]];
-			ABB_CHECK(h2d(a->spec, sub, st));
-			std::vector<ContigRec> recs2;
-			std::vector<unsigned> status2;
-			ABB_CHECK(run_extend(a, (unsigned)sub.size(), false, true, recs2, status2));
-			for (size_t i = 0; i < sub.size(); ++i)
-				if (status2[i] != 0) { // the serial walk itself ran out of scratch: end the round before this read
-					n_ok = std::min(n_ok, redo[i]);
-				}
-			std::vector<ContigRec> merged;
-			for (auto& r : recs)
-				if (!std::binary_search(redo.begin(), redo.end(), r.spec))
-					merged.push_back(r);
-			for (auto& r : recs2) {
-				r.spec = redo[r.spec];
-				merged.push_back(r);
-			}
-			recs.swap(merged);
-			ABB_CHECK(h2d(a->spec, spec, st)); // restore the full list for the replay
-			if (n_ok == 0) {
-				set_error("unitig scratch arena exhausted at %llu bytes", a->arena_size);
-				return ABB_ENOMEM;
-			}
-		}
-		layout_records(recs, n_ok, f->k, L);
-		ABB_CHECK(stage_contigs(a, recs, L));
-		te.stop();
 	}
-	if (n_ok < n_spec) {
-		// reads from the first failure on go back to the queue; speculate less next time.
-		// Candidates after the failed read that this round already labelled "visited" are re-examined
-		// when the scan resumes there (monotone, so the label will be the same): undo the bookkeeping.
-		const unsigned failed_read = spec[n_ok];
-		const size_t p = std::lower_bound(cand.begin(), cand.end(), failed_read) - cand.begin();
-		for (size_t i = p; i < *cursor; ++i)
-			if (a->out_codes[cand[i]] == RC_ALL_KMERS_VISITED) {
-				a->out_codes[cand[i]] = RC_CANDIDATE;
-				--a->counters.visited_reads;
-			}
-		*cursor = p;
-		a->spec_target = std::max(1u, n_ok);
-		spec.resize(n_ok);
+	for (unsigned i = 0; i < r.n_spec; ++i)
+		if (status[i] != 0) {
+			r.n_ok = i;
+			break;
+		}
+	if (r.n_ok == 0) {
+		if (status[0] & (walk_fail_bit(WALK_FAIL_LOOK_FULL) | walk_fail_bit(WALK_FAIL_FRAMES_FULL)))
+			set_error("graph traversal exceeded the per-warp scratch bounds (lookAhead %u / trueBranch %u frames)", kLookCap, kFrameCap);
+		else
+			set_error("unitig scratch arena exhausted at %llu bytes", a->arena_size);
+		return ABB_ENOMEM;
 	}
+	return ABB_OK;
+}
 
-	const unsigned nc = (unsigned)recs.size();
-	const std::vector<unsigned>& spec_cbeg = L.spec_cbeg;
-	const std::vector<unsigned>& clen = L.clen;
-	const std::vector<uint64_t>& coffs = L.coffs;
-	std::vector<uint8_t> rcode(n_ok), caccept(nc);
-	std::vector<unsigned> ccov(nc);
-	std::vector<uint64_t> hoff(nc + 1, 0); // where each accepted unitig lands in `seqs`
-	std::vector<char> seqs;
-	a->st_contigs_tried += nc;
-	{
-		PhaseTimer tr(a, &a->ms_replay);
-		ABB_CHECK(a->rcode.reserve(n_ok));
-		ABB_CHECK(a->caccept.reserve(nc + 1));
-		ABB_CHECK(a->ccov.reserve(nc + 1));
-		ABB_CHECK(ensure_endset(a, 2ull * nc));
-		a->ends_upper += 2ull * nc;
-		ReplayIO io;
-		io.spec = a->spec.p;
-		io.spec_cbeg = a->spec_cbeg.p;
-		io.n_spec = n_ok;
-		io.slot_offs = a->slot_offs.p;
-		io.h0 = a->h0.p;
-		io.cslot = a->cslot.p;
-		io.ch0 = a->ch0.p;
-		io.clen = a->clen.p;
-		io.cseq = a->cseq.p;
-		io.coffs = a->coffs.p;
-		io.care = a->solid->d_care.p;
-		io.rcode = a->rcode.p;
-		io.caccept = a->caccept.p;
-		io.ccov = a->ccov.p;
-		EndSet ends = { a->d_ends.p, a->ends_cap, a->d_ends_n.p };
-		if (nc) {
-			ABB_CUDA(cudaMemsetAsync(a->caccept.p, 0, nc, st));
-			ABB_CUDA(cudaMemsetAsync(a->ccov.p, 0, nc * sizeof(unsigned), st));
-		}
-		// one cooperative launch replays the whole round (k_replay_all)
-		{
-			std::vector<unsigned> big, big_s;
-			unsigned s_of = 0;
-			for (unsigned c = 0; c < nc; ++c) {
-				if (clen[c] - f->k + 1 < kBigContig)
-					continue;
-				while (spec_cbeg[s_of + 1] <= c)
-					++s_of;
-				big.push_back(c);
-				big_s.push_back(s_of);
-			}
-			ABB_CHECK(h2d(a->big_idx, big, st));
-			ABB_CHECK(h2d(a->big_spec, big_s, st));
-			static int replay_grid = 0;
-			if (replay_grid == 0) {
-				int per_sm = 0, sms = 0;
-				ABB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_replay_all, 1024, 0));
-				ABB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, f->device));
-				replay_grid = std::max(1, per_sm) * sms;
-			}
-			unsigned n_big = (unsigned)big.size(), nc_arg = nc, k_arg = f->k;
-			const unsigned* d_big = a->big_idx.p;
-			const unsigned* d_big_s = a->big_spec.p;
-			const uint8_t* d_counters = f->d_data.p;
-			uint8_t* d_bits = a->assembled->d_data.p;
-			void* params[] = { &io, &nc_arg, &d_big, &d_big_s, &n_big, &f->cfg, &k_arg, &d_counters, &d_bits, &ends };
-			ABB_CUDA(cudaLaunchCooperativeKernel((void*)k_replay_all, dim3((unsigned)replay_grid), dim3(1024), params, 0, st));
-			++a->st_launches;
-		}
-		ABB_CUDA(cudaGetLastError());
-		ABB_CUDA(cudaMemcpyAsync(rcode.data(), a->rcode.p, n_ok, cudaMemcpyDeviceToHost, st));
-		if (nc) {
-			ABB_CUDA(cudaMemcpyAsync(caccept.data(), a->caccept.p, nc, cudaMemcpyDeviceToHost, st));
-			ABB_CUDA(cudaMemcpyAsync(ccov.data(), a->ccov.p, nc * sizeof(unsigned), cudaMemcpyDeviceToHost, st));
-		}
-		ABB_CUDA(cudaStreamSynchronize(st));
-		// only the unitigs that were printed travel back to the host
-		for (unsigned c = 0; c < nc; ++c)
-			hoff[c + 1] = hoff[c] + (caccept[c] ? clen[c] : 0);
-		seqs.resize(hoff[nc]);
-		for (unsigned c = 0; c < nc; ++c)
-			if (caccept[c])
-				ABB_CUDA(cudaMemcpyAsync(seqs.data() + hoff[c], a->cseq.p + coffs[c], clen[c], cudaMemcpyDeviceToHost, st));
-		ABB_CUDA(cudaStreamSynchronize(st));
-		tr.stop();
-	}
+/** repeat check on everything that was produced with tiles: a read one of whose paths repeats a vertex is to be redone */
+int check_repeats(abb_assembler* a, Round& r)
+{
+	if (!a->tiles_on || !a->d_tile_tab.p)
+		return ABB_OK;
+	cudaStream_t st = a->stream;
+	std::vector<unsigned>& redo = r.redo;
+	std::vector<ContigRec> keep;
+	for (auto& rec : r.recs)
+		if (rec.spec < r.n_ok && std::find(redo.begin(), redo.end(), rec.spec) == redo.end())
+			keep.push_back(rec);
+	r.recs.swap(keep);
+	layout_records(r.recs, r.n_ok, a->solid->k, r.L);
+	ABB_CHECK(stage_contigs(a, r.recs, r.L));
+	const unsigned nc = (unsigned)r.recs.size();
+	if (nc == 0)
+		return ABB_OK;
+	std::vector<uint64_t> tab_off(nc + 1, 0);
+	for (unsigned c = 0; c < nc; ++c)
+		tab_off[c + 1] = tab_off[c] + 2 * (r.L.cslot[c + 1] - r.L.cslot[c]) + 8;
+	const uint64_t tab = tab_off[nc];
+	ABB_CHECK(h2d(a->rep_off, tab_off, st));
+	ABB_CHECK(a->rep_tab.reserve(tab));
+	ABB_CHECK(a->rep_flag.reserve(nc));
+	StreamTimer tr = a->time_inner(&a->st.ms_repeat); // read on return, after the synchronise below
+	ABB_CUDA(cudaMemsetAsync(a->rep_tab.p, 0, tab * sizeof(unsigned long long), st));
+	ABB_CUDA(cudaMemsetAsync(a->rep_flag.p, 0, nc, st));
+	k_repeat_check<<<a->sms * 8, 256, 0, st>>>(a->recs_sorted.p, nc, a->cslot.p, a->ch0.p, a->rep_tab.p, a->rep_off.p, a->rep_flag.p);
+	ABB_CUDA(cudaGetLastError());
+	tr.end();
+	++a->st.launches;
+	std::vector<uint8_t> flag(nc);
+	ABB_CUDA(cudaMemcpyAsync(flag.data(), a->rep_flag.p, nc, cudaMemcpyDeviceToHost, st));
+	ABB_CUDA(cudaStreamSynchronize(st));
+	for (unsigned c = 0; c < nc; ++c)
+		if (flag[c] && (redo.empty() || redo.back() != r.recs[c].spec) &&
+		    std::find(redo.begin(), redo.end(), r.recs[c].spec) == redo.end())
+			redo.push_back(r.recs[c].spec);
+	return ABB_OK;
+}
 
-	// ---- collect
+/** the exact vertex-by-vertex K4 for the reads to redo; their records replace what the tiled walk gave for them */
+int serial_fallback(abb_assembler* a, Round& r)
+{
+	cudaStream_t st = a->stream;
+	std::vector<unsigned>& redo = r.redo;
+	redo.erase(std::remove_if(redo.begin(), redo.end(), [&](unsigned i) { return i >= r.n_ok; }), redo.end());
+	if (redo.empty())
+		return ABB_OK;
+	std::sort(redo.begin(), redo.end());
+	a->st.serial_fallbacks += redo.size();
+	std::vector<unsigned> sub(redo.size());
+	for (size_t i = 0; i < redo.size(); ++i)
+		sub[i] = r.spec[redo[i]];
+	ABB_CHECK(h2d(a->spec, sub, st));
+	std::vector<ContigRec> recs2;
+	std::vector<unsigned> status2;
+	ABB_CHECK(run_extend(a, (unsigned)sub.size(), false, true, recs2, status2));
+	for (size_t i = 0; i < sub.size(); ++i)
+		if (status2[i] != 0) // the serial walk itself ran out of scratch: end the round before this read
+			r.n_ok = std::min(r.n_ok, redo[i]);
+	std::vector<ContigRec> merged;
+	for (auto& rec : r.recs)
+		if (!std::binary_search(redo.begin(), redo.end(), rec.spec))
+			merged.push_back(rec);
+	for (auto& rec : recs2) {
+		rec.spec = redo[rec.spec];
+		merged.push_back(rec);
+	}
+	r.recs.swap(merged);
+	ABB_CHECK(h2d(a->spec, r.spec, st)); // restore the full list for the replay
+	if (r.n_ok == 0) {
+		set_error("unitig scratch arena exhausted at %llu bytes", a->arena_size);
+		return ABB_ENOMEM;
+	}
+	return ABB_OK;
+}
+
+/** reads from the first failure on go back to the queue; speculate less next time.
+ *  Candidates after the failed read that this round already labelled "visited" are re-examined
+ *  when the scan resumes there (monotone, so the label will be the same): undo the bookkeeping. */
+void hand_back_failed(abb_assembler* a, const std::vector<unsigned>& cand, size_t* cursor, Round& r)
+{
+	if (r.n_ok == r.n_spec)
+		return;
+	const unsigned failed_read = r.spec[r.n_ok];
+	const size_t p = std::lower_bound(cand.begin(), cand.end(), failed_read) - cand.begin();
+	for (size_t i = p; i < *cursor; ++i)
+		if (a->out_codes[cand[i]] == RC_ALL_KMERS_VISITED) {
+			a->out_codes[cand[i]] = RC_CANDIDATE;
+			--a->counters.visited_reads;
+		}
+	*cursor = p;
+	a->spec_target = std::max(1u, r.n_ok);
+	r.spec.resize(r.n_ok);
+}
+
+/** K5: one cooperative launch replays the whole round (k_replay_all); its decisions and the printed unitigs come back */
+int replay(abb_assembler* a, Round& r)
+{
+	abb_filter* f = a->solid;
+	cudaStream_t st = a->stream;
+	const unsigned nc = (unsigned)r.recs.size(), n_ok = r.n_ok;
+	const std::vector<unsigned>& clen = r.L.clen;
+	r.rcode.resize(n_ok);
+	r.caccept.resize(nc);
+	r.ccov.resize(nc);
+	r.hoff.assign(nc + 1, 0);
+	a->st.contigs_tried += nc;
+	StreamTimer tr = a->time_phase(&a->st.ms_replay);
+	ABB_CHECK(a->rcode.reserve(n_ok));
+	ABB_CHECK(a->caccept.reserve(nc + 1));
+	ABB_CHECK(a->ccov.reserve(nc + 1));
+	ABB_CHECK(ensure_endset(a, 2ull * nc));
+	a->ends_upper += 2ull * nc;
+	ReplayIO io;
+	io.spec = a->spec.p;
+	io.spec_cbeg = a->spec_cbeg.p;
+	io.n_spec = n_ok;
+	io.slot_offs = a->slot_offs.p;
+	io.h0 = a->h0.p;
+	io.cslot = a->cslot.p;
+	io.ch0 = a->ch0.p;
+	io.clen = a->clen.p;
+	io.cseq = a->cseq.p;
+	io.coffs = a->coffs.p;
+	io.care = a->solid->d_care.p;
+	io.rcode = a->rcode.p;
+	io.caccept = a->caccept.p;
+	io.ccov = a->ccov.p;
+	EndSet ends = { a->d_ends.p, a->ends_cap, a->d_ends_n.p };
+	if (nc) {
+		ABB_CUDA(cudaMemsetAsync(a->caccept.p, 0, nc, st));
+		ABB_CUDA(cudaMemsetAsync(a->ccov.p, 0, nc * sizeof(unsigned), st));
+	}
+	std::vector<unsigned> big, big_s; // the unitigs of kBigContig k-mers and more, and the read each belongs to
+	unsigned s_of = 0;
+	for (unsigned c = 0; c < nc; ++c) {
+		if (clen[c] - f->k + 1 < kBigContig)
+			continue;
+		while (r.L.spec_cbeg[s_of + 1] <= c)
+			++s_of;
+		big.push_back(c);
+		big_s.push_back(s_of);
+	}
+	ABB_CHECK(h2d(a->big_idx, big, st));
+	ABB_CHECK(h2d(a->big_spec, big_s, st));
+	unsigned n_big = (unsigned)big.size(), nc_arg = nc, k_arg = f->k;
+	const unsigned* d_big = a->big_idx.p;
+	const unsigned* d_big_s = a->big_spec.p;
+	const uint8_t* d_counters = f->d_data.p;
+	uint8_t* d_bits = a->assembled->d_data.p;
+	void* params[] = { &io, &nc_arg, &d_big, &d_big_s, &n_big, &f->cfg, &k_arg, &d_counters, &d_bits, &ends };
+	ABB_CUDA(cudaLaunchCooperativeKernel((void*)k_replay_all, dim3(a->replay_grid), dim3(1024), params, 0, st));
+	++a->st.launches;
+	ABB_CUDA(cudaGetLastError());
+	ABB_CUDA(cudaMemcpyAsync(r.rcode.data(), a->rcode.p, n_ok, cudaMemcpyDeviceToHost, st));
+	if (nc) {
+		ABB_CUDA(cudaMemcpyAsync(r.caccept.data(), a->caccept.p, nc, cudaMemcpyDeviceToHost, st));
+		ABB_CUDA(cudaMemcpyAsync(r.ccov.data(), a->ccov.p, nc * sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+	}
+	ABB_CUDA(cudaStreamSynchronize(st));
+	// only the unitigs that were printed travel back to the host
+	for (unsigned c = 0; c < nc; ++c)
+		r.hoff[c + 1] = r.hoff[c] + (r.caccept[c] ? clen[c] : 0);
+	r.seqs.resize(r.hoff[nc]);
+	for (unsigned c = 0; c < nc; ++c)
+		if (r.caccept[c])
+			ABB_CUDA(cudaMemcpyAsync(r.seqs.data() + r.hoff[c], a->cseq.p + r.L.coffs[c], clen[c], cudaMemcpyDeviceToHost, st));
+	ABB_CUDA(cudaStreamSynchronize(st));
+	return ABB_OK;
+}
+
+/** the replay's decisions become read codes, contigs and trace rows; then adapt the amount of speculation */
+void collect(abb_assembler* a, const Round& r)
+{
+	const std::vector<unsigned>& clen = r.L.clen;
 	unsigned wasted = 0;
-	for (unsigned s = 0; s < n_ok; ++s) {
-		a->out_codes[spec[s]] = rcode[s];
-		if (rcode[s] == RC_ALL_KMERS_VISITED) {
+	for (unsigned s = 0; s < r.n_ok; ++s) {
+		a->out_codes[r.spec[s]] = r.rcode[s];
+		if (r.rcode[s] == RC_ALL_KMERS_VISITED) {
 			++a->counters.visited_reads;
 			++wasted;
 			continue;
 		}
-		for (unsigned c = spec_cbeg[s]; c < spec_cbeg[s + 1]; ++c) {
+		for (unsigned c = r.L.spec_cbeg[s]; c < r.L.spec_cbeg[s + 1]; ++c) {
 			if (a->params.reserved & 1u) { // ContigRecord (bloom-dbg.h:186-254): every contig that reached outputContig
 				abb_trace_row tr;
-				tr.contig_id = caccept[c] ? a->counters.contig_id : ~0ULL;
-				tr.seed_read = a->reads_seen + spec[s];
+				tr.contig_id = r.caccept[c] ? a->counters.contig_id : ~0ULL;
+				tr.seed_read = a->reads_seen + r.spec[s];
 				tr.length = clen[c];
-				tr.seed_pos = recs[c].seed_pos;
-				tr.left_n = recs[c].left_n;
-				tr.right_n = recs[c].right_n;
-				tr.left_code = recs[c].left;
-				tr.right_code = recs[c].right;
-				tr.redundant = caccept[c] ? 0 : 1;
+				tr.seed_pos = r.recs[c].seed_pos;
+				tr.left_n = r.recs[c].left_n;
+				tr.right_n = r.recs[c].right_n;
+				tr.left_code = r.recs[c].left;
+				tr.right_code = r.recs[c].right;
+				tr.redundant = r.caccept[c] ? 0 : 1;
 				tr.pad = 0;
 				a->out_trace.push_back(tr);
 			}
-			if (!caccept[c])
+			if (!r.caccept[c])
 				continue;
 			abb_contig oc;
-			oc.seed_read = a->reads_seen + spec[s];
+			oc.seed_read = a->reads_seen + r.spec[s];
 			oc.seq_offset = a->out_seqs.size();
 			oc.length = clen[c];
-			oc.coverage = ccov[c];
+			oc.coverage = r.ccov[c];
 			a->out_contigs.push_back(oc);
-			a->out_seqs.insert(a->out_seqs.end(), seqs.begin() + hoff[c], seqs.begin() + hoff[c] + clen[c]);
+			a->out_seqs.insert(a->out_seqs.end(), r.seqs.begin() + r.hoff[c], r.seqs.begin() + r.hoff[c] + clen[c]);
 			a->out_seqs.push_back('\0');
 			++a->counters.contig_id;
 			a->counters.bases_assembled += clen[c];
 		}
 	}
-	a->st_wasted += wasted;
-	// adapt the amount of speculation: grow while most speculated reads were really needed
-	if (n_ok == n_spec) {
-		if (wasted * 2 <= n_ok)
+	a->st.wasted_reads += wasted;
+	// grow while most speculated reads were really needed
+	if (r.n_ok == r.n_spec) {
+		if (wasted * 2 <= r.n_ok)
 			a->spec_target = std::min(kMaxSpec, a->spec_target * 2);
-		else if (wasted * 20 > n_ok * 19)
+		else if (wasted * 20 > r.n_ok * 19)
 			a->spec_target = std::max(kMinSpec, a->spec_target / 2);
 	}
-	(void)n_reads;
+}
+
+/** one speculation round over the candidates from *cursor on (the loop body of the pipeline at the top of this file);
+ *  appends the accepted contigs */
+int speculate_round(abb_assembler* a, const std::vector<unsigned>& cand, size_t* cursor)
+{
+	Round r;
+	ABB_CHECK(scan_uncovered(a, cand, cursor, r)); // K3b
+	if (r.spec.empty())
+		return ABB_OK;
+	++a->st.rounds;
+	a->st.speculated_reads += r.n_spec;
+	{
+		StreamTimer te = a->time_phase(&a->st.ms_extend);
+		ABB_CHECK(extend_tiled(a, r)); // K4
+		ABB_CHECK(check_repeats(a, r));
+		ABB_CHECK(serial_fallback(a, r)); // K4 again, without tiles
+		layout_records(r.recs, r.n_ok, a->solid->k, r.L);
+		ABB_CHECK(stage_contigs(a, r.recs, r.L)); // K1
+	}
+	hand_back_failed(a, cand, cursor, r);
+	ABB_CHECK(replay(a, r)); // K5
+	collect(a, r);
 	return ABB_OK;
 }
 
@@ -2037,6 +2045,12 @@ int abb_assembler_create(abb_assembler** out, abb_filter* solid, const abb_assem
 	ABB_CHECK(abb_filter_create(&assembled, ABB_BIT, solid->size, solid->H, solid->k, 0, "", solid->device));
 	a->assembled.reset(assembled);
 	a->stream = solid->stream; // one stream carries pass 1 and pass 2 of a filter
+	a->sms = sm_count();
+	int per_sm = 0;
+	ABB_DISPATCH_KW(a->kw, ABB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_make_tiles<KW>, kWalkWarps * 32, 0)));
+	a->tile_ctas = a->sms * (unsigned)std::max(1, per_sm);
+	ABB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_replay_all, 1024, 0));
+	a->replay_grid = a->sms * (unsigned)std::max(1, per_sm);
 	for (Event* e : { &a->ev[0], &a->ev[1], &a->ev2[0], &a->ev2[1] })
 		ABB_CUDA(cudaEventCreate(e->out()));
 	ABB_CHECK(a->d_arena_top.alloc(1));
@@ -2063,23 +2077,20 @@ static int hash_and_classify(abb_assembler* a, const uint8_t* d_bases, const uin
 	abb_filter* f = a->solid;
 	cudaStream_t st = a->stream;
 	uint64_t total = 0;
-	ABB_CHECK(compute_slot_offsets(f->k, d_offs, n_reads, a->slot_offs, a->scan_tmp, st, &total, &a->st_launches));
+	ABB_CHECK(compute_slot_offsets(f->k, d_offs, n_reads, a->slot_offs, a->scan_tmp, st, &total, &a->st.launches));
 	ABB_CHECK(a->h0.reserve(total + 1));
 	ABB_CHECK(a->valid.reserve(total + 1));
 	ABB_CHECK(a->codes.reserve(n_reads));
 	if (total)
 		ABB_CHECK(launch_hash(f->k, f->d_care.p, d_bases, d_offs, a->slot_offs.p, 0, n_reads, 0, a->h0.p, a->valid.p, st,
-		                      &a->st_launches));
+		                      &a->st.launches));
 	*total_out = total;
 	if (!classify)
 		return ABB_OK;
-	int sms = 132;
-	cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, f->device);
 	// K3a is pure per read: with a communicator every rank classifies its contiguous slice of the batch and the codes
 	// are all-gathered
-	const unsigned world = a->comm ? (unsigned)abb_comm_world(a->comm) : 1u, rank = a->comm ? (unsigned)abb_comm_rank(a->comm) : 0u;
-	const uint64_t lo = rank * n_reads / world, up = (rank + 1) * n_reads / world;
-	const unsigned grid = (unsigned)std::min<uint64_t>(blocks_for(std::max<uint64_t>(up - lo, 1), kWalkWarps), (uint64_t)sms * 8);
+	const auto [lo, up] = slice_of(n_reads, a->rank(), a->world());
+	const unsigned grid = std::min(blocks_for(std::max<uint64_t>(up - lo, 1), kWalkWarps), a->sms * 8);
 	ABB_CHECK(ensure_scratch(a, grid * kWalkWarps));
 	const WalkCfg w = walk_cfg(a);
 	if (up > lo)
@@ -2087,8 +2098,8 @@ static int hash_and_classify(abb_assembler* a, const uint8_t* d_bases, const uin
 		                                                                        up - lo, w, f->cfg, a->look.p, (int)a->params.read_log,
 		                                                                        a->codes.p + lo)));
 	ABB_CUDA(cudaGetLastError());
-	++a->st_launches;
-	if (world > 1)
+	++a->st.launches;
+	if (a->world() > 1)
 		ABB_CHECK(allgather_slices(a, a->codes.p + lo, n_reads, a->codes.p));
 	return ABB_OK;
 }
@@ -2100,25 +2111,25 @@ static int process_batch(abb_assembler* a, const uint8_t* d_bases, const uint64_
 	struct Total {
 		abb_assembler* a;
 		std::chrono::steady_clock::time_point t0;
-		~Total() { a->ms_total += std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count(); }
+		~Total() { a->st.ms_total += std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count(); }
 	} total_guard{ a, t_begin };
-	abb_filter* f = a->solid;
 	cudaStream_t st = a->stream;
 	a->cur_bases = d_bases;
 	a->cur_offs = d_offs;
-	PhaseTimer tc(a, &a->ms_classify);
 	uint64_t total = 0;
-	const bool external = a->ext_codes != nullptr;
-	ABB_CHECK(hash_and_classify(a, d_bases, d_offs, n_reads, !external, &total));
-	if (external) { // classification done elsewhere (sharded over several GPUs): take it as is
-		ABB_REQUIRE(a->ext_n == n_reads, "abb_assembler_set_codes: %llu codes for %llu reads", (unsigned long long)a->ext_n,
-		            (unsigned long long)n_reads);
-		ABB_CUDA(cudaMemcpyAsync(a->codes.p, a->ext_codes, n_reads, cudaMemcpyDeviceToDevice, st));
-		a->ext_codes = nullptr;
+	{
+		StreamTimer tc = a->time_phase(&a->st.ms_classify);
+		const bool external = a->ext_codes != nullptr;
+		ABB_CHECK(hash_and_classify(a, d_bases, d_offs, n_reads, !external, &total));
+		if (external) { // classification done elsewhere (sharded over several GPUs): take it as is
+			ABB_REQUIRE(a->ext_n == n_reads, "abb_assembler_set_codes: %llu codes for %llu reads", (unsigned long long)a->ext_n,
+			            (unsigned long long)n_reads);
+			ABB_CUDA(cudaMemcpyAsync(a->codes.p, a->ext_codes, n_reads, cudaMemcpyDeviceToDevice, st));
+			a->ext_codes = nullptr;
+		}
+		ABB_CUDA(cudaMemcpyAsync(a->out_codes.data(), a->codes.p, n_reads, cudaMemcpyDeviceToHost, st));
+		ABB_CUDA(cudaStreamSynchronize(st));
 	}
-	ABB_CUDA(cudaMemcpyAsync(a->out_codes.data(), a->codes.p, n_reads, cudaMemcpyDeviceToHost, st));
-	ABB_CUDA(cudaStreamSynchronize(st));
-	tc.stop();
 
 	const auto t_cand = std::chrono::steady_clock::now();
 	// candidate list = indices of the reads classified RC_CANDIDATE, compacted on the device
@@ -2139,15 +2150,15 @@ static int process_batch(abb_assembler* a, const uint8_t* d_bases, const uint64_
 			ABB_CUDA(cudaMemcpyAsync(cand.data(), a->cand.p, (size_t)nc * sizeof(unsigned), cudaMemcpyDeviceToHost, st));
 		ABB_CUDA(cudaStreamSynchronize(st));
 	}
-	a->ms_cand += std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t_cand).count();
+	a->st.ms_cand += std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t_cand).count();
 	a->counters.solid_reads += cand.size();
-	a->st_candidates += cand.size();
+	a->st.candidates += cand.size();
 	if (!cand.empty())
 		ABB_CHECK(produce_tiles(a, n_reads, total));
 
 	size_t cursor = 0;
 	while (cursor < cand.size())
-		ABB_CHECK(speculate_round(a, cand, &cursor, n_reads));
+		ABB_CHECK(speculate_round(a, cand, &cursor));
 
 	a->counters.reads_processed += n_reads;
 	a->reads_seen += n_reads;
@@ -2204,25 +2215,7 @@ int abb_assembler_process_reads_dev(abb_assembler* a, const char* d_bases, const
 int abb_assembler_stats(const abb_assembler* a, abb_assembly_stats* out)
 {
 	ABB_REQUIRE(a && out, "NULL argument");
-	out->rounds = a->st_iterations;
-	out->speculated_reads = a->st_speculated;
-	out->wasted_reads = a->st_wasted;
-	out->candidates = a->st_candidates;
-	out->contigs_tried = a->st_contigs_tried;
-	out->launches = a->st_launches;
-	out->ms_classify = a->ms_classify;
-	out->ms_visited = a->ms_visited;
-	out->ms_extend = a->ms_extend;
-	out->ms_replay = a->ms_replay;
-	out->ms_tiles = a->ms_tiles;
-	out->ms_walk = a->ms_walk;
-	out->ms_total = a->ms_total;
-	out->ms_cand = a->ms_cand;
-	out->ms_stage = a->ms_stage;
-	out->ms_repeat = a->ms_repeat;
-	out->markers = a->st_markers;
-	out->tiles = a->st_tiles;
-	out->serial_fallbacks = a->st_fallbacks;
+	*out = a->st;
 	return ABB_OK;
 }
 
@@ -2234,12 +2227,11 @@ int abb_assembler_classify_dev(abb_assembler* a, const char* d_bases, const uint
 	ABB_REQUIRE(d_bases && d_offsets && d_codes, "NULL buffer");
 	ABB_CUDA(cudaSetDevice(a->solid->device));
 	ABB_CUDA(cudaStreamSynchronize(a->solid->stream));
-	PhaseTimer tc(a, &a->ms_classify);
+	StreamTimer tc = a->time_phase(&a->st.ms_classify);
 	uint64_t total = 0;
 	ABB_CHECK(hash_and_classify(a, (const uint8_t*)d_bases, d_offsets, n_reads, true, &total));
 	ABB_CUDA(cudaMemcpyAsync(d_codes, a->codes.p, n_reads, cudaMemcpyDeviceToDevice, a->stream));
 	ABB_CUDA(cudaStreamSynchronize(a->stream));
-	tc.stop();
 	return ABB_OK;
 }
 
@@ -2272,9 +2264,7 @@ int abb_assembler_reset(abb_assembler* a)
 	a->counters = abb_assembly_counters{};
 	a->reads_seen = 0;
 	a->spec_target = 512;
-	a->st_iterations = a->st_speculated = a->st_wasted = a->st_launches = a->st_candidates = a->st_contigs_tried = 0;
-	a->st_markers = a->st_tiles = a->st_fallbacks = 0;
-	a->ms_classify = a->ms_visited = a->ms_extend = a->ms_replay = a->ms_tiles = a->ms_walk = a->ms_stage = a->ms_repeat = a->ms_total = a->ms_cand = 0;
+	a->st = abb_assembly_stats{};
 	a->out_contigs.clear();
 	a->out_seqs.clear();
 	a->out_codes.clear();

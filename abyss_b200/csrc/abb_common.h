@@ -118,6 +118,31 @@ struct SyncOnExit {
 	~SyncOnExit() { cudaStreamSynchronize(s); }
 };
 
+/** Adds the CUDA-event time of a stretch of a stream to *acc.  The stretch starts at construction and ends at end(), or
+ *  where the scope is left, on every return path, if end() was not called.  The time is read when the scope is left,
+ *  after waiting for the end event: a timer whose end() is followed by a stream synchronise waits for nothing. */
+struct StreamTimer {
+	cudaEvent_t e0, e1;
+	cudaStream_t s;
+	float* acc;
+	bool ended = false;
+	StreamTimer(cudaEvent_t e0_, cudaEvent_t e1_, cudaStream_t s_, float* acc_) : e0(e0_), e1(e1_), s(s_), acc(acc_) { cudaEventRecord(e0, s); }
+	StreamTimer(const StreamTimer&) = delete;
+	void end()
+	{
+		cudaEventRecord(e1, s);
+		ended = true;
+	}
+	~StreamTimer()
+	{
+		if (!ended)
+			end();
+		float ms = 0;
+		if (cudaEventSynchronize(e1) == cudaSuccess && cudaEventElapsedTime(&ms, e0, e1) == cudaSuccess)
+			*acc += ms;
+	}
+};
+
 /** hands a finished handle to the C caller, whose abb_*_destroy owns it from then on */
 template <typename T>
 int hand_over(std::unique_ptr<T>& h, T** out)

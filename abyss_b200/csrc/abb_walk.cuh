@@ -371,6 +371,17 @@ ABB_HD FrameView frame_unpack(uint64_t m)
 
 ABB_HD unsigned ctz4(unsigned m) { return (m & 1) ? 0 : (m & 2) ? 1 : (m & 4) ? 2 : 3; }
 
+/** Why a walk was abandoned: the value handed to Ctx::fail().  A context that reports to the host (WarpCtx, KonCtx) keeps
+ *  the set of reasons as a mask of walk_fail_bit(); k_extend stores that mask as the read's status, 0 = walked to the end. */
+enum WalkFail : unsigned {
+	WALK_FAIL_NO_CODE = 0,     // k_extend only: the walk returned "not ok" although no fail() was recorded
+	WALK_FAIL_LOOK_FULL = 1,   // lookAhead visited more than kLookCap vertices
+	WALK_FAIL_FRAMES_FULL = 2, // trueBranch recursed deeper than kFrameCap frames
+	WALK_FAIL_ARENA = 3,       // Ctx::alloc found the unitig arena exhausted
+	WALK_FAIL_TILE_CYCLE = 4,  // the tile chain came back to a tile already spliced: walk this read vertex by vertex
+};
+ABB_HD constexpr unsigned walk_fail_bit(WalkFail why) { return 1u << why; }
+
 /**
  * Ctx concept (device: WarpCtx in abb_assemble.cu; host emulation: tests/host_walk):
  *   unsigned k, trim; RollTab rt;
@@ -381,7 +392,7 @@ ABB_HD unsigned ctz4(unsigned m) { return (m & 1) ? 0 : (m & 2) ? 1 : (m & 4) ? 
  *   void sync()                      make lane-0 writes visible to the warp
  *   bool find64(const uint64_t* a, unsigned n, uint64_t key, unsigned stride_words)   cooperative linear search
  *   uint8_t* alloc(uint64_t bytes)   arena bump allocation, zero-filled iff zero==true; nullptr when exhausted
- *   void fail(unsigned why), bool failed()   record an overflow; the walk of this read is abandoned and retried by the host
+ *   void fail(unsigned why), bool failed()   record why (a WalkFail) the walk of this read is abandoned; the host retries it
  *   void copy8(dst, src, n), copy8_rev(dst, src, n)   cooperative byte copies (rev: dst[i] = src[n-1-i])
  *   void rehash(old, oldcap, new, newcap)              cooperative PathSet growth
  *   bool tiles_enabled(); const TileRec* tile_lookup(key, cls); const TileRec* tile_at(idx); void prefetch(const void*);
@@ -432,7 +443,7 @@ ABB_HD bool look_ahead(Ctx& c, const V& start, Dir dir, unsigned limit)
 			continue;
 		}
 		if (nvis >= kLookCap) {
-			c.fail(1);
+			c.fail(WALK_FAIL_LOOK_FULL);
 			return true;
 		}
 		c.wr64(c.look + nvis++, hv);
@@ -485,7 +496,7 @@ ABB_HD bool true_branch(Ctx& c, const V& u, Dir dir, unsigned base, unsigned tri
 				if (c.find64(&c.frames[0].hv, sp, hv, 2) || f.depth + 1 >= trim_i)
 					return true;
 				if (sp >= kFrameCap) {
-					c.fail(2);
+					c.fail(WALK_FAIL_FRAMES_FULL);
 					return true;
 				}
 				const unsigned nm = c.neighbors(cur);
@@ -534,7 +545,7 @@ ABB_HD bool true_branch(Ctx& c, const V& u, Dir dir, unsigned base, unsigned tri
 			if (c.find64(&c.frames[0].hv, sp, hv, 2))
 				return true;
 			if (sp >= kFrameCap) {
-				c.fail(2);
+				c.fail(WALK_FAIL_FRAMES_FULL);
 				return true;
 			}
 			const unsigned nm = c.neighbors(cur);
@@ -952,7 +963,7 @@ ABB_HD ExtCode extend_dir(Ctx& c, Vtx<KW>& head, Dir dir, unsigned* psize, ByteV
 				if (n) {
 					const uint32_t ti = c.tile_index(T);
 					if (ti == brent_tortoise) { // the same tile again: a cycle the splice cannot see; walk this read without tiles
-						c.fail(4);
+						c.fail(WALK_FAIL_TILE_CYCLE);
 						*ok = false;
 						return ER_DEAD_END;
 					}

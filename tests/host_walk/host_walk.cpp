@@ -112,7 +112,7 @@ struct HostCtx {
 	void fail(unsigned why)
 	{
 		fail_ = true;
-		if (why == 4)
+		if (why == abb::WALK_FAIL_TILE_CYCLE)
 			tile_cycle = true;
 		else
 			fprintf(stderr, "host_walk: scratch overflow %u\n", why);

@@ -29,7 +29,7 @@ class InsertStats(C.Structure):
                 ("deferred", C.c_uint64), ("launches", C.c_uint64),
                 ("ms_hash", C.c_float), ("ms_insert", C.c_float), ("ms_commit", C.c_float),
                 ("commit_launches", C.c_uint64), ("commit_slots", C.c_uint64), ("drains", C.c_uint64),
-                ("drained_slots", C.c_uint64)]
+                ("drained_slots", C.c_uint64), ("graph_launches", C.c_uint64), ("ms_graph", C.c_float)]
 
 
 class Contig(C.Structure):
@@ -62,6 +62,10 @@ class AssemblyCounters(C.Structure):
 
 class SuccInfo(C.Structure):
     _fields_ = [("hash", C.c_uint64 * 4), ("mask", C.c_uint8), ("pad", C.c_uint8 * 7)]
+
+
+class NbrInfo(C.Structure):
+    _fields_ = [("self", C.c_uint64), ("hash", C.c_uint64 * 8), ("attr", C.c_uint32), ("mask", C.c_uint8), ("pad", C.c_uint8 * 3)]
 
 
 class OverlapEdge(C.Structure):
@@ -141,6 +145,7 @@ SIGNATURES = {
     "abb_contains_reads": (C.c_int, [_vp, _vp, _vp, C.c_uint64, _vp, _vp, C.c_uint64, _u64p]),
     "abb_trim_reads": (C.c_int, [_vp, _vp, _vp, C.c_uint64, C.c_uint, _vp, _vp]),
     "abb_successors": (C.c_int, [_vp, _vp, C.c_uint64, C.c_uint, _vp, _vp, _vp]),
+    "abb_graph_neighbors": (C.c_int, [_vp, _vp, C.c_uint64, _vp, C.c_uint, _vp]),
     "abb_overlap_create": (C.c_int, [C.POINTER(_vp), C.c_int]),
     "abb_overlap_destroy": (C.c_int, [_vp]),
     "abb_overlap_build": (C.c_int, [_vp, _vp, _vp, C.c_uint64, C.c_uint, C.c_uint, C.c_int, C.POINTER(C.POINTER(OverlapEdge)), _u64p]),
@@ -618,3 +623,17 @@ def successors(filt: "Filter", kmers, max_chain: int = 1):
     for i in range(n):
         out.append(([(info[i * max_chain + s].mask, list(info[i * max_chain + s].hash)) for s in range(ln[i])], self_h[i]))
     return out
+
+
+def graph_neighbors(graph: "Filter", kmers, attrs=()):
+    """in- and out-edges of graph vertices and their attribute filters (abb_graph_neighbors; `abyss-bloom graph`): for every k-mer
+    a dict with its canonical hash `self`, `hash` = the canonical hashes of its successors u[1:]+b and predecessors b+u[:-1]
+    (b = A, C, G, T), `mask` = the bits of those the graph contains and `attr` = the bits of the filters of `attrs` that contain
+    the k-mer."""
+    lib = load()
+    ks = [s.encode() if isinstance(s, str) else bytes(s) for s in kmers]
+    n = len(ks)
+    out = (NbrInfo * n)()
+    handles = (_vp * max(1, len(attrs)))(*[a.handle for a in attrs])
+    check(lib.abb_graph_neighbors(graph.handle, b"".join(ks), n, handles, len(attrs), out))
+    return [{"self": o.self, "hash": list(o.hash), "mask": o.mask, "attr": o.attr} for o in out]

@@ -1351,6 +1351,74 @@ int abb_successors(abb_filter* f, const char* kmers, uint64_t n, unsigned max_ch
 	return ABB_OK;
 }
 
+/** k-mers per k_graph_neighbors launch of abb_graph_neighbors: bounds its staging to 12.5 MiB of k-mers (k = 192) and 5 MiB of
+ *  results, reused from call to call */
+constexpr uint64_t kNbrPiece = 1 << 16;
+
+/** ABB_ESTATE unless f is a bit or cascading filter without a spaced seed */
+static int require_bit_filter(const abb_filter* f, const char* what)
+{
+	if ((f->kind != ABB_BIT && f->kind != ABB_CASCADING) || !f->mask.empty()) {
+		set_error("abb_graph_neighbors: the %s must be a bit or cascading filter without a spaced seed", what);
+		return ABB_ESTATE;
+	}
+	return ABB_OK;
+}
+
+int abb_graph_neighbors(abb_filter* g, const char* kmers, uint64_t n, abb_filter* const* attr, unsigned n_attr, abb_nbr_info* out)
+{
+	ABB_CHECK(select_device(g ? g->device : 0));
+	ABB_REQUIRE(g, "NULL filter");
+	ABB_REQUIRE(n_attr <= kMaxAttrFilters, "at most %u attribute filters", kMaxAttrFilters);
+	ABB_REQUIRE(n_attr == 0 || attr, "NULL attribute filter list");
+	ABB_CHECK(require_bit_filter(g, "graph"));
+	NbrQuery q;
+	q.cfg = g->cfg;
+	q.rt = make_rolltab(g->k);
+	q.bits = g->level_data(g->levels - 1);
+	q.n_attr = n_attr;
+	for (unsigned a = 0; a < n_attr; ++a) {
+		const abb_filter* f = attr[a];
+		ABB_REQUIRE(f, "NULL attribute filter %u", a);
+		ABB_CHECK(require_bit_filter(f, "attribute filter"));
+		if (f->device != g->device || f->H > g->H) {
+			set_error("abb_graph_neighbors: attribute filter %u must live on the graph's device and use at most its %u hashes", a, g->H);
+			return ABB_ESTATE;
+		}
+		q.attr[a].bits = f->level_data(f->levels - 1);
+		q.attr[a].mod = f->cfg.mod;
+		q.attr[a].H = f->H;
+		ABB_CUDA(cudaStreamSynchronize(f->stream)); // its bits are read on the graph's stream
+	}
+	if (n == 0)
+		return ABB_OK;
+	ABB_REQUIRE(kmers && out, "NULL buffer");
+	const unsigned probes = nbr_lane_probes(q); // <= kMaxLaneProbes: H <= kMaxHashes, H_a <= H
+	const SyncOnExit sync = { g->stream };
+	ABB_CHECK(g->gq_kmers.reserve(std::min(n, kNbrPiece) * g->k));
+	ABB_CHECK(g->gq_nbr.reserve(std::min(n, kNbrPiece)));
+	for (uint64_t i0 = 0; i0 < n; i0 += kNbrPiece) {
+		const uint64_t m = std::min(kNbrPiece, n - i0);
+		ABB_CUDA(cudaMemcpyAsync(g->gq_kmers.p, kmers + i0 * g->k, m * g->k, cudaMemcpyHostToDevice, g->stream));
+		{
+			// with profiling on, the CUDA-event time of the launch alone (abb_insert_stats::ms_graph)
+			std::unique_ptr<StreamTimer> timer;
+			if (g->profile)
+				timer.reset(new StreamTimer(g->ev0, g->ev1, g->stream, &g->st.ms_graph));
+			const unsigned grid = std::min<unsigned>(blocks_for(m, 8), sm_count() * 8);
+			with_lane_probes(probes, [&](auto P) {
+				k_graph_neighbors<decltype(P)::value><<<grid, 256, 0, g->stream>>>(g->gq_kmers.p, m, q, g->gq_nbr.p);
+			});
+			ABB_CUDA(cudaGetLastError());
+		}
+		g->st.launches += 1;
+		g->st.graph_launches += 1;
+		ABB_CUDA(cudaMemcpyAsync(out + i0, g->gq_nbr.p, m * sizeof(abb_nbr_info), cudaMemcpyDeviceToHost, g->stream));
+		ABB_CUDA(cudaStreamSynchronize(g->stream)); // the staging is reused by the next piece
+	}
+	return ABB_OK;
+}
+
 int abb_hash_reads(unsigned k, const char* mask, const char* bases, const uint64_t* offsets, uint64_t n_reads,
                    uint64_t* out_h0, uint8_t* out_valid, uint64_t* n_slots_out, int device)
 {

@@ -232,6 +232,7 @@ struct abb_filter {
 	abb::DevBuf<abb_succ_info> gq_info;
 	abb::DevBuf<unsigned> gq_len;
 	abb::DevBuf<uint64_t> gq_self;
+	abb::DevBuf<abb_nbr_info> gq_nbr; // abb_graph_neighbors (gq_kmers holds its k-mers)
 
 	/** device bytes from one level to the next.  Bit and cascading levels start on 16-byte boundaries: bits_set ORs 4-byte words
 	 *  and k_popcount loads uint4, while size / 8 need only be a multiple of 1.  Counting filters have one level, and the

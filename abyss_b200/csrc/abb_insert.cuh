@@ -951,23 +951,15 @@ struct FilterProbe {
 	HashCfg cfg;
 	FilterView f;
 	unsigned threshold;
-	ABB_HD static unsigned ld(const uint8_t* p)
-	{
-#if defined(__CUDA_ARCH__)
-		return __ldcg(p);
-#else
-		return *p;
-#endif
-	}
 	ABB_HD bool operator()(uint64_t h0) const
 	{
 		bool ok = true;
 		for (unsigned i = 0; i < cfg.H; ++i) { // independent loads: issued back to back
 			const uint64_t p = nth_pos(h0, cfg, i);
 			if (KIND == 0)
-				ok &= ld(f.data + p) >= threshold;
+				ok &= ld_filter(f.data + p) >= threshold;
 			else
-				ok &= (ld(f.data + (uint64_t)(f.levels - 1) * f.level_stride + (p >> 3)) >> (p & 7)) & 1;
+				ok &= bit_at(f.data + (uint64_t)(f.levels - 1) * f.level_stride, p);
 		}
 		return ok;
 	}

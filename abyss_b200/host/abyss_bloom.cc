@@ -2,9 +2,9 @@
 //   build -t konnector (default; CityHash, -l levels, -L N=FILE, -w M/N windows, -h seed), -t counting
 //     (CountingBloomFilter<uint8_t>, the filter abyss-bloom-dbg loads with -i) and -t rolling-hash [-l LEVELS]
 //     (HashAgnosticCascadingBloom, last level serialised);
-//   union, intersect, info, compare, kmers (getKmers), trim on Konnector files, and info on the two BTL formats.
-// Output files and printed text are byte-compatible with the reference's.  `graph` is not implemented (DESIGN.md section 7):
-// it orders its output by a std::unordered_set.
+//   union, intersect, info, compare, kmers (getKmers), trim on Konnector files, info on the two BTL formats, and graph on
+//   rolling-hash (BTL bit) files.
+// Output files and printed text are byte-compatible with the reference's.
 //
 //   abyss-bloom build [-v] -k K [-b SIZE] [-h SEED] [-l LEVELS] [-L N=FILE] [-w M/N] [-t konnector|counting|rolling-hash] OUT.bloom READS...
 //   abyss-bloom union|intersect -k K OUT.bloom IN.bloom IN.bloom...
@@ -12,8 +12,10 @@
 //   abyss-bloom compare -k K [-m jaccard|forbes|czekanowski] A.bloom B.bloom    (exits with status 1, as the reference does)
 //   abyss-bloom kmers -k K [-r] [--fasta|--bed|--raw] IN.bloom READS
 //   abyss-bloom trim [-v...] -k K [-q N] IN.bloom READS... > trimmed.fq
+//   abyss-bloom graph [-v] -k K [-d N] (-R KMER | -f FASTA)... [-a ATTR:FASTA]... [-A ATTR:BLOOM]... IN.bloom > graph.dot
 #include "../../include/abyss_b200.h"
 #include "bloom_file.h"
+#include "bloom_graph.h"
 #include "reads.h"
 #include "trim.h"
 #include <getopt.h>
@@ -560,6 +562,224 @@ static int trim(int argc, char** argv)
 	return EXIT_SUCCESS;
 }
 
+/** the canonical hash, and whether `graph` contains it (null: not asked), of every k-mer window of a batch; valid[s] = 0 for a
+ *  window RollingHashIterator skips */
+static void hash_windows(unsigned k, abb_filter* graph, const ReadBatch& b, std::vector<uint64_t>& h0, std::vector<uint8_t>& valid,
+                         std::vector<uint8_t>& flag, int device)
+{
+	uint64_t slots = 0;
+	for (size_t r = 0; r < b.size(); ++r) {
+		const uint64_t len = b.offsets[r + 1] - b.offsets[r];
+		slots += len >= k ? len - k + 1 : 0;
+	}
+	h0.resize(slots);
+	valid.resize(slots);
+	flag.resize(slots);
+	check(abb_hash_reads(k, "", b.bases.data(), b.offsets.data(), b.size(), h0.data(), valid.data(), &slots, device), "hash");
+	if (graph)
+		check(abb_contains_reads(graph, b.bases.data(), b.offsets.data(), b.size(), flag.data(), nullptr, slots, &slots), "contains");
+}
+
+/** graph (Bloom/bloom.cc:984-1153): the GraphViz dump of the rolling-hash Bloom de Bruijn graph of FILE within -d steps of the
+ *  roots, in either direction; the search and its text are host::bloom_graph (bloom_graph.h), the lookups of each level one
+ *  abb_graph_neighbors call.  Where the reference asserts or reads past an array -- a root whose length is not k, a -k that is
+ *  not the file's, an -A filter with more hashes than the graph -- and for a root with a character other than A, C, G, T, this
+ *  command says why and exits with status 1 (DESIGN.md, section 3, K7b). */
+static int graph(int argc, char** argv)
+{
+	// parseGlobalOpts (bloom.cc:296-344): -k and -v up to the first option of the command
+	unsigned k = 0;
+	int verbose = 0, device = 0;
+	optind = 2;
+	for (int c, prev = optind; (c = getopt_long(argc, argv, kShortOpts, kLongOpts, NULL)) != -1; prev = optind) {
+		if (c == '?')
+			usage();
+		else if (c == 'k')
+			k = parse_num<unsigned>(c, optarg);
+		else if (c == 'v')
+			++verbose;
+		else if (c == OPT_HELP || c == OPT_VERSION) {
+			std::cerr << PROGRAM ": see the reference's abyss-bloom --help\n";
+			exit(EXIT_SUCCESS);
+		} else {
+			optind = prev;
+			break;
+		}
+	}
+	if (k == 0) {
+		std::cerr << PROGRAM ": missing mandatory option `-k'\n";
+		usage();
+	}
+	uint64_t maxDepth = k;
+	std::vector<std::pair<std::string, std::string>> fastaAttrs, bloomAttrs; // (attribute, file)
+	std::vector<std::string> roots, rootFastas;
+	for (int c; (c = getopt_long(argc, argv, kShortOpts, kLongOpts, NULL)) != -1;) {
+		std::istringstream arg(optarg != NULL ? optarg : "");
+		switch (c) {
+		case '?': usage(); break;
+		case 'a':
+		case 'A': {
+			std::string s;
+			arg >> s;
+			const size_t pos = s.find(':');
+			if (pos < s.length())
+				(c == 'a' ? fastaAttrs : bloomAttrs).emplace_back(s.substr(0, pos), s.substr(pos + 1));
+			else
+				arg.setstate(std::ios::failbit);
+		} break;
+		case 'd': arg >> maxDepth; break;
+		case 'f': {
+			std::string path;
+			arg >> path;
+			rootFastas.push_back(path);
+		} break;
+		case 'R': {
+			std::string kmer;
+			arg >> kmer;
+			roots.push_back(kmer);
+		} break;
+		case OPT_DEVICE: arg >> device; break;
+		default: break;
+		}
+		// any other option with an argument is refused here: its argument is left unread
+		if (optarg != NULL && (!arg.eof() || arg.fail())) {
+			std::cerr << PROGRAM ": invalid option: `-" << (char)c << optarg << "'\n";
+			exit(EXIT_FAILURE);
+		}
+	}
+	if (roots.empty() && rootFastas.empty()) {
+		std::cerr << PROGRAM ": must specify either --root or --root-fasta\n";
+		usage();
+	}
+	if (argc - optind != 1) {
+		std::cerr << PROGRAM ": missing arguments\n";
+		usage();
+	}
+	const std::string bloomPath = argv[optind];
+	// -d is read as a size_t and kept in RollingBloomDBGVisitor's unsigned m_maxDepth (RollingBloomDBGVisitor.h:38,170):
+	// 2^32 + d is d
+	const unsigned depth = (unsigned)maxDepth;
+	if (verbose)
+		std::cerr << "Loading main Bloom filter from `" << bloomPath << "'..." << std::endl;
+	BloomHeader h;
+	std::vector<uint8_t> raw;
+	read_bit_bloom(bloomPath, h, raw);
+	if (h.kmerSize != k) {
+		std::cerr << PROGRAM ": `" << bloomPath << "' holds " << h.kmerSize << "-mers, not the " << k << "-mers of -k\n";
+		exit(EXIT_FAILURE);
+	}
+	abb_filter* g = nullptr;
+	check(abb_filter_create(&g, ABB_BIT, h.size, h.hashNum, h.kmerSize, 0, "", device), "filter");
+	check(abb_filter_upload(g, 0, raw.data(), raw.size()), "upload");
+	ReadOpts ropt;
+	ropt.chastityFilter = g_chastity;
+	ropt.trimMasked = g_trimMasked;
+	ropt.qualityOffset = g_qualityOffset;
+	std::vector<uint64_t> h0;
+	std::vector<uint8_t> valid, flag;
+	// --fasta-attr: the k-mers of each file (bloom.cc:1060-1092)
+	std::vector<FastaAttr> fastaSets;
+	for (const auto& a : fastaAttrs) {
+		if (verbose)
+			std::cerr << "Loading k-mers from `" << a.second << "', to be annotated with '" << a.first << "'\n";
+		fastaSets.emplace_back(a.first, std::unordered_set<uint64_t>());
+		uint64_t count = 0, checkpoint = 0;
+		host::BatchStream stream({ a.second }, ropt, 1 << 20, 0, false);
+		while (const ReadBatch* b = stream.next()) {
+			hash_windows(k, nullptr, *b, h0, valid, flag, device);
+			uint64_t s = 0;
+			for (size_t r = 0; r < b->size(); ++r) {
+				const uint64_t len = b->offsets[r + 1] - b->offsets[r];
+				for (uint64_t i = 0; len >= k && i + k <= len; ++i, ++s)
+					if (valid[s]) {
+						fastaSets.back().second.insert(h0[s]);
+						++count;
+					}
+				for (; verbose && count >= checkpoint; checkpoint += 10000)
+					std::cerr << "Loaded " << checkpoint << " k-mers\n";
+			}
+		}
+		if (verbose)
+			std::cerr << "Loaded " << count << " k-mers in total\n";
+	}
+	// --bloom-attr (bloom.cc:1094-1110)
+	std::vector<abb_filter*> attrFilters;
+	std::vector<std::string> attrNames;
+	for (const auto& a : bloomAttrs) {
+		if (verbose)
+			std::cerr << "Loading Bloom filter from `" << a.second << "', to be annotated with '" << a.first << "'\n";
+		BloomHeader ah;
+		std::vector<uint8_t> araw;
+		read_bit_bloom(a.second, ah, araw);
+		if (ah.hashNum > h.hashNum) {
+			std::cerr << PROGRAM ": `" << a.second << "' uses " << ah.hashNum << " hash functions, more than the " << h.hashNum
+			          << " of the graph's filter\n";
+			exit(EXIT_FAILURE);
+		}
+		abb_filter* f = nullptr;
+		check(abb_filter_create(&f, ABB_BIT, ah.size, ah.hashNum, ah.kmerSize, 0, "", device), "filter");
+		check(abb_filter_upload(f, 0, araw.data(), araw.size()), "upload");
+		attrFilters.push_back(f);
+		attrNames.push_back(a.first);
+		if (verbose) { // printRollingBloomStats (bloom.cc:469-476)
+			uint64_t nz = 0;
+			check(abb_filter_popcount(f, &nz, nullptr), "popcount");
+			std::cerr << "Bloom size (bits): " << ah.size << "\nBloom popcount (bits): " << nz << "\nBloom filter FPR: " << std::setprecision(3)
+			          << 100 * std::pow((double)nz / (double)ah.size, (double)ah.hashNum) << "%\n";
+		}
+	}
+	// -R, then -f (bloom.cc:1112-1137)
+	GraphRoots rootSet;
+	for (const std::string& r : roots) {
+		if (r.size() != k) {
+			std::cerr << PROGRAM ": root `" << r << "' is not a " << k << "-mer\n";
+			exit(EXIT_FAILURE);
+		}
+		if (r.find_first_not_of("ACGTacgt") != std::string::npos) {
+			std::cerr << PROGRAM ": root `" << r << "' has a character other than A, C, G, T\n";
+			exit(EXIT_FAILURE);
+		}
+	}
+	if (!roots.empty()) {
+		ReadBatch b;
+		for (const std::string& r : roots)
+			b.add("", r);
+		hash_windows(k, g, b, h0, valid, flag, device);
+		for (size_t i = 0; i < roots.size(); ++i)
+			if (flag[i])
+				rootSet.add(h0[i], roots[i].data(), k);
+	}
+	for (const std::string& path : rootFastas) {
+		host::BatchStream stream({ path }, ropt, 1 << 20, 0, false);
+		while (const ReadBatch* b = stream.next()) {
+			hash_windows(k, g, *b, h0, valid, flag, device);
+			uint64_t s = 0;
+			for (size_t r = 0; r < b->size(); ++r) {
+				const uint64_t len = b->offsets[r + 1] - b->offsets[r];
+				for (uint64_t i = 0; len >= k && i + k <= len; ++i, ++s)
+					if (valid[s] && flag[s])
+						rootSet.add(h0[s], b->bases.data() + b->offsets[r] + i, k);
+			}
+		}
+	}
+	std::ostringstream buf;
+	host::bloom_graph(
+	    k, depth, rootSet, fastaSets, attrNames,
+	    [&](const char* kmers, uint64_t n, abb_nbr_info* out) {
+		    check(abb_graph_neighbors(g, kmers, n, attrFilters.data(), (unsigned)attrFilters.size(), out), "graph");
+		    if (buf.tellp() > (8 << 20)) {
+			    std::cout << buf.str();
+			    buf.str("");
+		    }
+	    },
+	    buf);
+	std::cout << buf.str() << std::flush;
+	for (abb_filter* f : attrFilters)
+		abb_filter_destroy(f);
+	abb_filter_destroy(g);
+	return EXIT_SUCCESS;
+}
+
 int main(int argc, char** argv)
 {
 	const std::string cmd = argc >= 2 ? argv[1] : "";
@@ -583,10 +803,8 @@ int main(int argc, char** argv)
 		return kmers(argc, argv);
 	if (cmd == "trim")
 		return trim(argc, argv);
-	if (cmd == "graph") {
-		std::cerr << PROGRAM ": `" << cmd << "' is not implemented on the GPU (DESIGN.md section 7)\n";
-		usage();
-	}
+	if (cmd == "graph")
+		return graph(argc, argv);
 	if (cmd != "build") {
 		std::cerr << PROGRAM ": unrecognized command: `" << cmd << "'" << std::endl;
 		usage();

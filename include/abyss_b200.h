@@ -317,6 +317,22 @@ typedef struct abb_succ_info {
 int abb_successors(abb_filter* f, const char* kmers, uint64_t n, unsigned max_chain, abb_succ_info* out, unsigned* out_len,
                    uint64_t* self_hash);
 
+/* ---- neighbourhoods of graph vertices, for `abyss-bloom graph` (Bloom/bloom.cc:984-1153; RollingBloomDBG.h:300-445;
+ * RollingBloomDBGVisitor::discover_vertex): for each of n k-mers (n * k characters, ACGT in either case) its canonical ntHash,
+ * the canonical hashes of its 4 successors u[1:] + b and 4 predecessors b + u[:-1] (b = A, C, G, T), which of them the graph
+ * contains, and which of n_attr (<= 32) attribute filters contain the k-mer itself.  The graph is the last level of an ABB_BIT or
+ * ABB_CASCADING filter; an attribute filter is an ABB_BIT or ABB_CASCADING filter (last level) on the graph's device with at most
+ * the graph's number of hashes, tested, as the reference does, with the first H of the graph's hash values modulo its own size.
+ * Any other filter, or a spaced seed, is ABB_ESTATE.  Any n: the batch is processed in pieces of bounded device memory. */
+typedef struct abb_nbr_info {
+	uint64_t self;    /* canonical hash of the k-mer (vertex identity) */
+	uint64_t hash[8]; /* [b]: successor u[1:] + b, [4 + b]: predecessor b + u[:-1] */
+	uint32_t attr;    /* bit a: attribute filter a contains the k-mer */
+	uint8_t mask;     /* bit j: the graph contains neighbour j */
+	uint8_t pad[3];
+} abb_nbr_info;
+int abb_graph_neighbors(abb_filter* graph, const char* kmers, uint64_t n, abb_filter* const* attr, unsigned n_attr, abb_nbr_info* out);
+
 /* ---- the next stage: contig overlap graph (AdjList/AdjList.cpp:140-291; bin/abyss-pe:577 runs it on the unitig FASTA) ----
  * Vertices are ContigNode indices (Common/ContigNode.h): 2*i = contig i as given, 2*i+1 = its reverse complement.
  * Edges u -> v: the last `overlap` bases of u equal the first `overlap` bases of v; distance = -overlap.
@@ -355,9 +371,11 @@ typedef struct abb_insert_stats {
 	uint64_t commit_slots;    /* k-mer slots those launches applied */
 	uint64_t drains;          /* serial drains that did work, and the slots they replayed */
 	uint64_t drained_slots;
+	uint64_t graph_launches;  /* k_graph_neighbors launches (abb_graph_neighbors) */
+	float ms_graph;           /* with profiling on: summed CUDA-event time of those launches */
 } abb_insert_stats;
 int abb_filter_insert_stats(abb_filter* f, abb_insert_stats* out, int reset);
-/* time launches of the Bloom-insert window kernel with CUDA events (bench.py roofline) */
+/* time launches of the Bloom-insert window kernel (bench.py roofline) and of k_graph_neighbors with CUDA events */
 int abb_filter_set_profiling(abb_filter* f, int on);
 /* the cudaStream_t all work of this filter (and of an assembler created on it) is issued to */
 void* abb_filter_stream(abb_filter* f);

@@ -106,7 +106,6 @@ SIGNATURES = {
     "abb_mincount_hashes": (C.c_int, [_vp, _vp, C.c_uint64, _vp]),
     "abb_hash_reads": (C.c_int, [C.c_uint, C.c_char_p, _vp, _vp, C.c_uint64, _vp, _vp, _u64p, C.c_int]),
     "abb_hash_reads_dev": (C.c_int, [_vp, _vp, _vp, C.c_uint64, _vp, _vp, C.c_uint64, _u64p]),
-    "abb_insert_h0_dev": (C.c_int, [_vp, _vp, C.c_uint64]),
     "abb_comm_unique_id": (C.c_int, [_vp]),
     "abb_comm_create": (C.c_int, [C.POINTER(_vp), C.c_int, C.c_int, _vp, C.c_int]),
     "abb_comm_destroy": (C.c_int, [_vp]),
@@ -117,7 +116,6 @@ SIGNATURES = {
     "abb_filter_resident_reads": (C.c_int, [_vp, C.POINTER(_vp), C.POINTER(_vp), _u64p]),
     "abb_filter_allgather": (C.c_int, [_vp, _vp]),
     "abb_comm_allgather_bytes": (C.c_int, [_vp, _vp, C.c_uint64, _vp]),
-    "abb_comm_allreduce_max_u8": (C.c_int, [_vp, _vp, C.c_uint64, _vp]),
     "abb_comm_exchange_bytes": (C.c_int, [_vp, _vp, C.c_uint64, _vp, _u64p, _u64p, _vp]),
     "abb_filter_device_ptr": (_vp, [_vp, C.c_int]),
     "abb_filter_download": (C.c_int, [_vp, C.c_int, _vp, C.c_uint64]),
@@ -130,8 +128,6 @@ SIGNATURES = {
     "abb_assembler_process_reads_dev": (C.c_int, [_vp, _vp, _vp, C.c_uint64, C.POINTER(C.POINTER(Contig)), _u64p, C.POINTER(C.c_char_p)]),
     "abb_assembler_stats": (C.c_int, [_vp, C.POINTER(AssemblyStats)]),
     "abb_assembler_reset": (C.c_int, [_vp]),
-    "abb_assembler_classify_dev": (C.c_int, [_vp, _vp, _vp, C.c_uint64, _vp]),
-    "abb_assembler_set_codes": (C.c_int, [_vp, _vp, C.c_uint64]),
     "abb_assembler_counters": (C.c_int, [_vp, C.POINTER(AssemblyCounters)]),
     "abb_assembler_set_counters": (C.c_int, [_vp, C.POINTER(AssemblyCounters)]),
     "abb_assembler_read_results": (C.c_int, [_vp, C.POINTER(_u8p), _u64p]),
@@ -237,9 +233,6 @@ class Comm:
 
     def allgather_bytes(self, d_buf_ptr: int, bytes_per_rank: int, stream: int = 0):
         check(self._lib.abb_comm_allgather_bytes(self._h, _vp(d_buf_ptr), bytes_per_rank, _vp(stream)))
-
-    def allreduce_max_u8(self, d_buf_ptr: int, n: int, stream: int = 0):
-        check(self._lib.abb_comm_allreduce_max_u8(self._h, _vp(d_buf_ptr), n, _vp(stream)))
 
     def close(self):
         if self._h:
@@ -380,9 +373,6 @@ class Filter:
     def allgather(self, comm: "Comm"):
         check(self._lib.abb_filter_allgather(self._h, comm.handle))
 
-    def insert_h0_dev(self, d_h0_ptr: int, n: int):
-        check(self._lib.abb_insert_h0_dev(self._h, _vp(d_h0_ptr), n))
-
     def device_ptr(self, level: int = -1) -> int:
         return self._lib.abb_filter_device_ptr(self._h, level) or 0
 
@@ -479,12 +469,6 @@ class Assembler:
         """multi-GPU pass 2: shard classification, candidate scans and tile production over the ranks of `comm`"""
         self._comm = comm
         check(self._lib.abb_assembler_set_comm(self._h, comm.handle if comm is not None else None))
-
-    def classify_dev(self, d_bases_ptr: int, d_offs_ptr: int, n_reads: int, d_codes_ptr: int):
-        check(self._lib.abb_assembler_classify_dev(self._h, _vp(d_bases_ptr), _vp(d_offs_ptr), n_reads, _vp(d_codes_ptr)))
-
-    def set_codes(self, d_codes_ptr: int, n_reads: int):
-        check(self._lib.abb_assembler_set_codes(self._h, _vp(d_codes_ptr), n_reads))
 
     def stats(self) -> AssemblyStats:
         st = AssemblyStats()

@@ -268,7 +268,7 @@ static int ordered_insert(abb_filter* f, const uint64_t* d_hashes, const uint8_t
 	a.f = view_of(f);
 	a.age_off = (unsigned)(age_windows_for(W) * W);
 	a.drain_age = a.age_off / 3 * 2;
-	a.ctl = reinterpret_cast<InsertCtl*>(f->d_ctl.p);
+	a.ctl = f->d_ctl.p;
 	a.stats = f->d_stats.p;
 	uint64_t* sorted = f->d_carry.p + 2 * cap;
 	// the maps, both tag tables and the control block start clean
@@ -428,6 +428,38 @@ int compute_slot_offsets(unsigned k, const uint64_t* d_offs, uint64_t n_reads, D
 	return ABB_OK;
 }
 
+int check_read_batch(const char* bases, const uint64_t* offsets, uint64_t n_reads, const char* noun)
+{
+	if (n_reads == 0)
+		return ABB_OK;
+	ABB_REQUIRE(bases && offsets, "NULL %s buffers", noun);
+	ABB_REQUIRE(offsets[0] == 0, "offsets[0] must be 0");
+	return ABB_OK;
+}
+
+int stage_read_batch(const char* bases, const uint64_t* offsets, uint64_t n_reads, DevBuf<uint8_t>& d_bases, DevBuf<uint64_t>& d_offs,
+                     cudaStream_t stream)
+{
+	if (n_reads == 0)
+		return ABB_OK;
+	const uint64_t n_bases = offsets[n_reads];
+	ABB_CHECK(d_bases.reserve(n_bases + 16));
+	ABB_CHECK(d_offs.reserve(n_reads + 1));
+	ABB_CUDA(cudaMemcpyAsync(d_offs.p, offsets, (n_reads + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, stream));
+	if (bases)
+		ABB_CUDA(cudaMemcpyAsync(d_bases.p, bases, n_bases, cudaMemcpyHostToDevice, stream));
+	return ABB_OK;
+}
+
+int resolve_level(const abb_filter* f, int level, unsigned* out)
+{
+	if (level < 0)
+		level = (int)f->levels - 1;
+	ABB_REQUIRE((unsigned)level < f->levels, "level %d out of range", level);
+	*out = (unsigned)level;
+	return ABB_OK;
+}
+
 static int sharded_ordered_insert(abb_filter* f, abb_comm* c, const uint64_t* d_h0, const uint8_t* d_valid, uint64_t n_slots);
 
 /** a host-to-device copy of the bases that is still in flight, in pieces of `piece` bytes on f->copy_stream
@@ -487,7 +519,7 @@ static int insert_reads_dev(abb_filter* f, const uint8_t* d_bases, const uint64_
 		ABB_CUDA(cudaMemcpyAsync(&slot_at[i], f->slot_offs.p + bounds[i], sizeof(uint64_t), cudaMemcpyDeviceToHost, f->stream));
 	ABB_CUDA(cudaStreamSynchronize(f->stream));
 
-	ABB_CUDA(cudaMemsetAsync(f->d_stats.p + 3, 0, sizeof(unsigned long long), f->stream));
+	ABB_CUDA(cudaMemsetAsync(f->d_stats.p + kStatInsertKmers, 0, sizeof(unsigned long long), f->stream));
 	for (size_t c = 0; c + 1 < bounds.size(); ++c) {
 		const uint64_t r0 = bounds[c], r1 = bounds[c + 1];
 		const uint64_t slots = slot_at[c + 1] - slot_at[c];
@@ -500,7 +532,8 @@ static int insert_reads_dev(abb_filter* f, const uint8_t* d_bases, const uint64_
 		ABB_CUDA(cudaEventRecord(f->ev0, f->stream));
 		ABB_CHECK(launch_hash(f->k, f->d_care.p, d_bases, d_offs, f->slot_offs.p, r0, r1, slot_at[c], f->h0.p, f->valid.p, f->stream,
 		                      &f->st.launches));
-		k_count_valid<<<std::min<unsigned>(blocks_for(slots, 256), sm_count() * 8), 256, 0, f->stream>>>(f->valid.p, slots, f->d_stats.p + 3);
+		k_count_valid<<<std::min<unsigned>(blocks_for(slots, 256), sm_count() * 8), 256, 0, f->stream>>>(f->valid.p, slots,
+		                                                                                                  f->d_stats.p + kStatInsertKmers);
 		f->st.launches += 1;
 		ABB_CUDA(cudaEventRecord(f->ev1, f->stream));
 		if (comm)
@@ -519,7 +552,7 @@ static int insert_reads_dev(abb_filter* f, const uint8_t* d_bases, const uint64_
 		f->st.slots += slots;
 	}
 	unsigned long long nk = 0;
-	ABB_CUDA(cudaMemcpyAsync(&nk, f->d_stats.p + 3, sizeof nk, cudaMemcpyDeviceToHost, f->stream));
+	ABB_CUDA(cudaMemcpyAsync(&nk, f->d_stats.p + kStatInsertKmers, sizeof nk, cudaMemcpyDeviceToHost, f->stream));
 	ABB_CUDA(cudaStreamSynchronize(f->stream));
 	f->st.kmers += nk;
 	if (n_kmers_out)
@@ -623,8 +656,7 @@ static int sharded_ordered_insert(abb_filter* f, abb_comm* c, const uint64_t* d_
 	const unsigned drain_age = age_off / 3 * 2;
 	const uint64_t cap = 3 * (W + kCarryLanes) / 2; // two lists in the allocation of three (no drain list is needed here)
 	uint64_t* carry[2] = { f->d_carry.p, f->d_carry.p + cap };
-	ShardCtl* ctl = reinterpret_cast<ShardCtl*>(f->d_ctl.p);
-	unsigned* d_nout = f->d_ctl.p + 4; // [n_out]; the ctl block has 8 words
+	ShardCtl* ctl = f->d_shard_ctl.p;
 	const size_t map_bytes = std::max<size_t>(f->map_entries / 4, 256);
 	ConflictMap maps[2] = { { f->d_map[0], f->map_entries - 1 }, { f->d_map[1], f->map_entries - 1 } };
 	const uint64_t chunk = shard_chunk(f->size, (unsigned)c->world);
@@ -634,10 +666,9 @@ static int sharded_ordered_insert(abb_filter* f, abb_comm* c, const uint64_t* d_
 	{
 		ShardCtl init;
 		init.n_pending = 0;
-		init.pad = 0;
+		init.n_out = 0;
 		init.lo_pending = ~0ULL;
 		ABB_CUDA(cudaMemcpyAsync(ctl, &init, sizeof init, cudaMemcpyHostToDevice, st));
-		ABB_CUDA(cudaMemsetAsync(d_nout, 0, 4 * sizeof(unsigned), st));
 	}
 	ABB_CUDA(cudaMemsetAsync(f->d_map[0], 0, 3 * map_bytes, st)); // the maps start clean
 	unsigned n_in = 0; // host copy of the carry length (identical on every rank)
@@ -676,9 +707,9 @@ static int sharded_ordered_insert(abb_filter* f, abb_comm* c, const uint64_t* d_
 				cudaEventRecord(f->prof_ev[f->prof_used++], st);
 				f->prof_slots += n;
 			}
-			k_sh_compact<<<1, kDrainThreads, 0, st>>>(f->d_slotbits.p, lo_slot, w0 + std::max<uint64_t>(n, 1), carry[1 - in], ctl, d_nout);
+			k_sh_compact<<<1, kDrainThreads, 0, st>>>(f->d_slotbits.p, lo_slot, w0 + std::max<uint64_t>(n, 1), carry[1 - in], ctl, &ctl->n_out);
 			unsigned h_n = 0;
-			ABB_CUDA(cudaMemcpyAsync(&h_n, d_nout, sizeof h_n, cudaMemcpyDeviceToHost, st));
+			ABB_CUDA(cudaMemcpyAsync(&h_n, &ctl->n_out, sizeof h_n, cudaMemcpyDeviceToHost, st));
 			// the oldest pending slot bounds the priorities
 			ABB_CUDA(cudaMemcpyAsync(&oldest, carry[1 - in], sizeof oldest, cudaMemcpyDeviceToHost, st));
 			ABB_CUDA(cudaStreamSynchronize(st));
@@ -720,10 +751,7 @@ static int sharded_ordered_insert(abb_filter* f, abb_comm* c, const uint64_t* d_
 	}
 	ABB_CHECK(drain(n_slots, 0));
 	ABB_CUDA(cudaGetLastError());
-	ABB_CHECK(fold_profile(f));
-	// leave the shared control block in the single-GPU layout
-	ABB_CUDA(cudaMemsetAsync(f->d_ctl.p, 0, 8 * sizeof(unsigned), st));
-	return ABB_OK;
+	return fold_profile(f);
 }
 
 } // namespace abb
@@ -819,10 +847,11 @@ static int alloc_filter(std::unique_ptr<abb_filter> f, abb_filter** out)
 	// slack: the in-place all-gather of position shards rounds each shard up to 16 bytes (abb_filter_allgather)
 	ABB_CHECK(f->d_data.alloc(f->level_stride() * levels + 4096));
 	ABB_CUDA(cudaMemsetAsync(f->d_data.p, 0, f->level_stride() * levels, f->stream));
-	ABB_CHECK(f->d_ctl.alloc(8));
-	ABB_CUDA(cudaMemsetAsync(f->d_ctl.p, 0, 8 * sizeof(unsigned), f->stream));
-	ABB_CHECK(f->d_stats.alloc(8));
-	ABB_CUDA(cudaMemsetAsync(f->d_stats.p, 0, 8 * sizeof(unsigned long long), f->stream));
+	ABB_CHECK(f->d_ctl.alloc(1));
+	ABB_CUDA(cudaMemsetAsync(f->d_ctl.p, 0, sizeof(InsertCtl), f->stream));
+	ABB_CHECK(f->d_shard_ctl.alloc(1));
+	ABB_CHECK(f->d_stats.alloc(kStatWords));
+	ABB_CUDA(cudaMemsetAsync(f->d_stats.p, 0, kStatWords * sizeof(unsigned long long), f->stream));
 	if (!f->mask.empty()) {
 		std::vector<uint8_t> care(k);
 		for (unsigned i = 0; i < k; ++i)
@@ -938,26 +967,20 @@ int abb_insert_reads(abb_filter* f, const char* bases, const uint64_t* offsets, 
 		*n_kmers_out = 0;
 	if (n_reads == 0)
 		return ABB_OK;
-	ABB_REQUIRE(bases && offsets, "NULL read buffers");
-	ABB_REQUIRE(offsets[0] == 0, "offsets[0] must be 0");
+	ABB_CHECK(check_read_batch(bases, offsets, n_reads));
 	const uint64_t n_bases = offsets[n_reads];
 	ABB_CUDA(cudaSetDevice(f->device));
-	ABB_CHECK(f->bases.reserve(n_bases + 16));
-	ABB_CHECK(f->offs.reserve(n_reads + 1));
-	ABB_CUDA(cudaMemcpyAsync(f->offs.p, offsets, (n_reads + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, f->stream));
-	f->resident_reads = n_reads;
-	if (f->kind == ABB_KONNECTOR) {
-		ABB_CUDA(cudaMemcpyAsync(f->bases.p, bases, n_bases, cudaMemcpyHostToDevice, f->stream));
-		return kon_insert_reads_dev(f, f->bases.p, f->offs.p, n_reads, n_kmers_out);
-	}
 	// The bases travel in pieces on a second stream; chunk c of the insert only waits for the pieces that hold its reads, so
 	// the copy of the rest hides behind the hashing and inserting of the earlier chunks (with pinned host memory; a pageable
 	// buffer makes cudaMemcpyAsync synchronous and the order is simply copy, then insert).  One piece: one copy up front.
 	constexpr uint64_t kPiece = 256ULL << 20;
-	if (n_bases <= kPiece) {
-		ABB_CUDA(cudaMemcpyAsync(f->bases.p, bases, n_bases, cudaMemcpyHostToDevice, f->stream));
+	const bool in_pieces = f->kind != ABB_KONNECTOR && n_bases > kPiece;
+	ABB_CHECK(stage_read_batch(in_pieces ? nullptr : bases, offsets, n_reads, f->bases, f->offs, f->stream));
+	f->resident_reads = n_reads;
+	if (f->kind == ABB_KONNECTOR)
+		return kon_insert_reads_dev(f, f->bases.p, f->offs.p, n_reads, n_kmers_out);
+	if (!in_pieces)
 		return insert_reads_dev(f, f->bases.p, f->offs.p, n_reads, n_kmers_out);
-	}
 	if (!f->copy_stream)
 		ABB_CUDA(cudaStreamCreateWithFlags(f->copy_stream.out(), cudaStreamNonBlocking));
 	if (f->kind != ABB_BIT)
@@ -1012,16 +1035,9 @@ int abb_insert_reads_sharded(abb_filter* f, abb_comm* c, const char* bases, cons
 	}
 	if (n_kmers_out)
 		*n_kmers_out = 0;
-	ABB_REQUIRE(n_reads == 0 || (bases && offsets), "NULL read buffers");
-	ABB_REQUIRE(n_reads == 0 || offsets[0] == 0, "offsets[0] must be 0");
+	ABB_CHECK(check_read_batch(bases, offsets, n_reads));
 	ABB_CUDA(cudaSetDevice(f->device));
-	if (n_reads) {
-		const uint64_t n_bases = offsets[n_reads];
-		ABB_CHECK(f->bases.reserve(n_bases + 16));
-		ABB_CHECK(f->offs.reserve(n_reads + 1));
-		ABB_CUDA(cudaMemcpyAsync(f->bases.p, bases, n_bases, cudaMemcpyHostToDevice, f->stream));
-		ABB_CUDA(cudaMemcpyAsync(f->offs.p, offsets, (n_reads + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, f->stream));
-	}
+	ABB_CHECK(stage_read_batch(bases, offsets, n_reads, f->bases, f->offs, f->stream));
 	f->resident_reads = n_reads;
 	return abb_insert_reads_sharded_dev(f, c, (const char*)f->bases.p, f->offs.p, n_reads, finalize, n_kmers_out);
 }
@@ -1048,21 +1064,6 @@ int abb_insert_hashes(abb_filter* f, const uint64_t* hashes, uint64_t n)
 	ABB_CHECK(ordered_insert<true>(f, f->lit.p, nullptr, n));
 	ABB_CUDA(cudaStreamSynchronize(f->stream));
 	f->st.kmers += n;
-	return ABB_OK;
-}
-
-int abb_insert_h0_dev(abb_filter* f, const uint64_t* d_h0, uint64_t n)
-{
-	ABB_REQUIRE(f, "NULL filter");
-	ABB_REQUIRE_NTHASH(f);
-	if (n == 0)
-		return ABB_OK;
-	ABB_REQUIRE(d_h0, "NULL hashes");
-	ABB_CUDA(cudaSetDevice(f->device));
-	ABB_CHECK(ordered_insert<false>(f, d_h0, nullptr, n));
-	ABB_CUDA(cudaStreamSynchronize(f->stream));
-	f->st.kmers += n;
-	f->st.slots += n;
 	return ABB_OK;
 }
 
@@ -1189,16 +1190,6 @@ int abb_comm_exchange_bytes(abb_comm* c, const void* d_send, uint64_t send_bytes
 	return ABB_OK;
 }
 
-int abb_comm_allreduce_max_u8(abb_comm* c, void* d_buf, uint64_t n, void* cuda_stream)
-{
-	ABB_REQUIRE(c && (d_buf || n == 0), "NULL argument");
-	if (c->world == 1 || n == 0)
-		return ABB_OK;
-	ABB_CUDA(cudaSetDevice(c->device));
-	ABB_NCCL(g_nccl.AllReduce(d_buf, d_buf, n, ncclUint8, ncclMax, c->comm, (cudaStream_t)cuda_stream));
-	return ABB_OK;
-}
-
 int abb_insert_reads_sharded_dev(abb_filter* f, abb_comm* c, const char* d_bases, const uint64_t* d_offsets, uint64_t n_reads,
                                  int finalize, uint64_t* n_kmers_out)
 {
@@ -1222,15 +1213,12 @@ int abb_insert_reads_sharded_dev(abb_filter* f, abb_comm* c, const char* d_bases
 
 void* abb_filter_device_ptr(abb_filter* f, int level)
 {
-	if (!f)
-		return nullptr;
-	if (level < 0)
-		level = (int)f->levels - 1;
-	if ((unsigned)level >= f->levels)
+	unsigned l = 0;
+	if (!f || resolve_level(f, level, &l) != ABB_OK)
 		return nullptr;
 	cudaSetDevice(f->device);
 	cudaStreamSynchronize(f->stream);
-	return f->level_data((unsigned)level);
+	return f->level_data(l);
 }
 
 static int query_hashes(abb_filter* f, const uint64_t* hashes, uint64_t n, uint8_t* out, bool want_min)
@@ -1269,18 +1257,13 @@ int abb_contains_reads(abb_filter* f, const char* bases, const uint64_t* offsets
 		*n_slots_out = 0;
 	if (n_reads == 0)
 		return ABB_OK;
-	ABB_REQUIRE(bases && offsets, "NULL read buffers");
-	ABB_REQUIRE(offsets[0] == 0, "offsets[0] must be 0");
+	ABB_CHECK(check_read_batch(bases, offsets, n_reads));
 	ABB_CUDA(cudaSetDevice(f->device));
-	const uint64_t n_bases = offsets[n_reads];
 	// own staging buffers: the batch a previous insert left resident (abb_filter_resident_reads) stays valid
 	DevBuf<uint8_t> d_bases;
 	DevBuf<uint64_t> d_offs;
-	ABB_CHECK(d_bases.reserve(n_bases + 16));
-	ABB_CHECK(d_offs.reserve(n_reads + 1));
 	const SyncOnExit sync = { f->stream }; // before the staging buffers are freed
-	ABB_CUDA(cudaMemcpyAsync(d_bases.p, bases, n_bases, cudaMemcpyHostToDevice, f->stream));
-	ABB_CUDA(cudaMemcpyAsync(d_offs.p, offsets, (n_reads + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, f->stream));
+	ABB_CHECK(stage_read_batch(bases, offsets, n_reads, d_bases, d_offs, f->stream));
 	uint64_t total = 0;
 	ABB_CHECK(compute_slot_offsets(f->k, d_offs.p, n_reads, f->slot_offs, f->scan_tmp, f->stream, &total, &f->st.launches));
 	if (n_slots_out)
@@ -1427,7 +1410,7 @@ int abb_hash_reads(unsigned k, const char* mask, const char* bases, const uint64
 		*n_slots_out = 0;
 	if (n_reads == 0)
 		return ABB_OK;
-	ABB_REQUIRE(bases && offsets, "NULL read buffers");
+	ABB_CHECK(check_read_batch(bases, offsets, n_reads));
 	ABB_CHECK(select_device(device));
 	std::string m = mask ? mask : "";
 	if (!m.empty()) {
@@ -1435,13 +1418,9 @@ int abb_hash_reads(unsigned k, const char* mask, const char* bases, const uint64
 		if (m.find('0') == std::string::npos)
 			m.clear();
 	}
-	const uint64_t n_bases = offsets[n_reads];
 	DevBuf<uint8_t> d_bases, d_valid, tmp, d_care;
 	DevBuf<uint64_t> d_offs, d_slot, d_h0;
-	ABB_CHECK(d_bases.reserve(n_bases + 16));
-	ABB_CHECK(d_offs.reserve(n_reads + 1));
-	ABB_CUDA(cudaMemcpy(d_bases.p, bases, n_bases, cudaMemcpyHostToDevice));
-	ABB_CUDA(cudaMemcpy(d_offs.p, offsets, (n_reads + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice));
+	ABB_CHECK(stage_read_batch(bases, offsets, n_reads, d_bases, d_offs, 0));
 	if (!m.empty()) {
 		std::vector<uint8_t> care(k);
 		for (unsigned i = 0; i < k; ++i)
@@ -1467,12 +1446,11 @@ int abb_hash_reads(unsigned k, const char* mask, const char* bases, const uint64
 static int level_ptr(abb_filter* f, int level, uint64_t nbytes, uint8_t** p)
 {
 	ABB_REQUIRE(f, "NULL filter");
-	if (level < 0)
-		level = (int)f->levels - 1;
-	ABB_REQUIRE((unsigned)level < f->levels, "level %d out of range", level);
+	unsigned l = 0;
+	ABB_CHECK(resolve_level(f, level, &l));
 	ABB_REQUIRE(nbytes == f->bytes_per_level, "buffer is %llu bytes, the filter level is %llu", (unsigned long long)nbytes,
 	            (unsigned long long)f->bytes_per_level);
-	*p = f->level_data((unsigned)level);
+	*p = f->level_data(l);
 	return ABB_OK;
 }
 
@@ -1520,14 +1498,15 @@ int abb_filter_popcount(abb_filter* f, uint64_t* nonzero, uint64_t* at_or_above_
 		return ABB_OK;
 	}
 	ABB_CUDA(cudaSetDevice(f->device));
-	ABB_CUDA(cudaMemsetAsync(f->d_stats.p + 4, 0, 2 * sizeof(unsigned long long), f->stream));
+	ABB_CUDA(cudaMemsetAsync(f->d_stats.p + kStatPopcount, 0, 2 * sizeof(unsigned long long), f->stream));
 	// bit / cascading: population of the LAST level (the one contains() consults)
 	const uint8_t* p = f->level_data(f->levels - 1);
-	k_popcount<<<sm_count() * 8, 256, 0, f->stream>>>(p, f->bytes_per_level, f->kind == ABB_COUNTING, f->threshold, f->d_stats.p + 4);
+	k_popcount<<<sm_count() * 8, 256, 0, f->stream>>>(p, f->bytes_per_level, f->kind == ABB_COUNTING, f->threshold,
+	                                                  f->d_stats.p + kStatPopcount);
 	f->st.launches += 1;
 	ABB_CUDA(cudaGetLastError());
 	unsigned long long h[2] = { 0, 0 };
-	ABB_CUDA(cudaMemcpyAsync(h, f->d_stats.p + 4, sizeof h, cudaMemcpyDeviceToHost, f->stream));
+	ABB_CUDA(cudaMemcpyAsync(h, f->d_stats.p + kStatPopcount, sizeof h, cudaMemcpyDeviceToHost, f->stream));
 	ABB_CUDA(cudaStreamSynchronize(f->stream));
 	if (nonzero)
 		*nonzero = h[0];
@@ -1542,18 +1521,18 @@ int abb_filter_insert_stats(abb_filter* f, abb_insert_stats* out, int reset)
 {
 	ABB_REQUIRE(f, "NULL filter");
 	ABB_CUDA(cudaSetDevice(f->device));
-	unsigned long long h[3] = { 0, 0, 0 };
+	unsigned long long h[kStatDrainedSlots + 1] = {}; // the words that accumulate over calls
 	ABB_CUDA(cudaMemcpyAsync(h, f->d_stats.p, sizeof h, cudaMemcpyDeviceToHost, f->stream));
 	ABB_CUDA(cudaStreamSynchronize(f->stream));
-	f->st.deferred = h[0];
-	f->st.drains = h[1] + f->sh_drains;
-	f->st.drained_slots = h[2];
+	f->st.deferred = h[kStatDeferred];
+	f->st.drains = h[kStatDrains] + f->sh_drains;
+	f->st.drained_slots = h[kStatDrainedSlots];
 	if (out)
 		*out = f->st;
 	if (reset) {
 		f->sh_drains = 0;
 		f->st = abb_insert_stats{};
-		ABB_CUDA(cudaMemsetAsync(f->d_stats.p, 0, 3 * sizeof(unsigned long long), f->stream));
+		ABB_CUDA(cudaMemsetAsync(f->d_stats.p, 0, sizeof h, f->stream));
 	}
 	return ABB_OK;
 }

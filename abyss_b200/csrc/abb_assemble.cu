@@ -1183,8 +1183,6 @@ struct abb_assembler {
 	int kw = 0;
 	RollTab rt; // per-k roll constants + spaced-seed positions
 	DevBuf<uint8_t> d_mpos;
-	const uint8_t* ext_codes = nullptr; // not owned: classification supplied by the caller for the next batch (device)
-	uint64_t ext_n = 0;
 	abb_comm* comm = nullptr;           // not owned; multi-GPU: classification, candidate scans and tile production are sharded over it
 	DevBuf<uint8_t> gather;             // all-gather staging (world x padded slice)
 	const uint8_t* cur_bases = nullptr; // not owned: device reads of the batch being processed
@@ -2070,9 +2068,8 @@ int abb_assembler_destroy(abb_assembler* a)
 	return ABB_OK;
 }
 
-/** slot offsets + K1 over the batch into a->h0 / a->valid, then (unless codes come from outside) K3a */
-static int hash_and_classify(abb_assembler* a, const uint8_t* d_bases, const uint64_t* d_offs, uint64_t n_reads, bool classify,
-                             uint64_t* total_out)
+/** slot offsets + K1 over the batch into a->h0 / a->valid, then K3a */
+static int hash_and_classify(abb_assembler* a, const uint8_t* d_bases, const uint64_t* d_offs, uint64_t n_reads, uint64_t* total_out)
 {
 	abb_filter* f = a->solid;
 	cudaStream_t st = a->stream;
@@ -2085,8 +2082,6 @@ static int hash_and_classify(abb_assembler* a, const uint8_t* d_bases, const uin
 		ABB_CHECK(launch_hash(f->k, f->d_care.p, d_bases, d_offs, a->slot_offs.p, 0, n_reads, 0, a->h0.p, a->valid.p, st,
 		                      &a->st.launches));
 	*total_out = total;
-	if (!classify)
-		return ABB_OK;
 	// K3a is pure per read: with a communicator every rank classifies its contiguous slice of the batch and the codes
 	// are all-gathered
 	const auto [lo, up] = slice_of(n_reads, a->rank(), a->world());
@@ -2119,14 +2114,7 @@ static int process_batch(abb_assembler* a, const uint8_t* d_bases, const uint64_
 	uint64_t total = 0;
 	{
 		StreamTimer tc = a->time_phase(&a->st.ms_classify);
-		const bool external = a->ext_codes != nullptr;
-		ABB_CHECK(hash_and_classify(a, d_bases, d_offs, n_reads, !external, &total));
-		if (external) { // classification done elsewhere (sharded over several GPUs): take it as is
-			ABB_REQUIRE(a->ext_n == n_reads, "abb_assembler_set_codes: %llu codes for %llu reads", (unsigned long long)a->ext_n,
-			            (unsigned long long)n_reads);
-			ABB_CUDA(cudaMemcpyAsync(a->codes.p, a->ext_codes, n_reads, cudaMemcpyDeviceToDevice, st));
-			a->ext_codes = nullptr;
-		}
+		ABB_CHECK(hash_and_classify(a, d_bases, d_offs, n_reads, &total));
 		ABB_CUDA(cudaMemcpyAsync(a->out_codes.data(), a->codes.p, n_reads, cudaMemcpyDeviceToHost, st));
 		ABB_CUDA(cudaStreamSynchronize(st));
 	}
@@ -2192,13 +2180,8 @@ int abb_assembler_process_reads(abb_assembler* a, const char* bases, const uint6
 	ABB_CHECK(begin_batch(a, n_reads, contigs, n_contigs, seqs));
 	if (n_reads == 0)
 		return ABB_OK;
-	ABB_REQUIRE(bases && offsets, "NULL read buffers");
-	ABB_REQUIRE(offsets[0] == 0, "offsets[0] must be 0");
-	const uint64_t n_bases = offsets[n_reads];
-	ABB_CHECK(a->bases.reserve(n_bases + 16));
-	ABB_CHECK(a->offs.reserve(n_reads + 1));
-	ABB_CUDA(cudaMemcpyAsync(a->bases.p, bases, n_bases, cudaMemcpyHostToDevice, a->stream));
-	ABB_CUDA(cudaMemcpyAsync(a->offs.p, offsets, (n_reads + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, a->stream));
+	ABB_CHECK(check_read_batch(bases, offsets, n_reads));
+	ABB_CHECK(stage_read_batch(bases, offsets, n_reads, a->bases, a->offs, a->stream));
 	return process_batch(a, a->bases.p, a->offs.p, n_reads, contigs, n_contigs, seqs);
 }
 
@@ -2216,30 +2199,6 @@ int abb_assembler_stats(const abb_assembler* a, abb_assembly_stats* out)
 {
 	ABB_REQUIRE(a && out, "NULL argument");
 	*out = a->st;
-	return ABB_OK;
-}
-
-int abb_assembler_classify_dev(abb_assembler* a, const char* d_bases, const uint64_t* d_offsets, uint64_t n_reads, uint8_t* d_codes)
-{
-	ABB_REQUIRE(a, "NULL assembler");
-	if (n_reads == 0)
-		return ABB_OK;
-	ABB_REQUIRE(d_bases && d_offsets && d_codes, "NULL buffer");
-	ABB_CUDA(cudaSetDevice(a->solid->device));
-	ABB_CUDA(cudaStreamSynchronize(a->solid->stream));
-	StreamTimer tc = a->time_phase(&a->st.ms_classify);
-	uint64_t total = 0;
-	ABB_CHECK(hash_and_classify(a, (const uint8_t*)d_bases, d_offsets, n_reads, true, &total));
-	ABB_CUDA(cudaMemcpyAsync(d_codes, a->codes.p, n_reads, cudaMemcpyDeviceToDevice, a->stream));
-	ABB_CUDA(cudaStreamSynchronize(a->stream));
-	return ABB_OK;
-}
-
-int abb_assembler_set_codes(abb_assembler* a, const uint8_t* d_codes, uint64_t n_reads)
-{
-	ABB_REQUIRE(a, "NULL assembler");
-	a->ext_codes = d_codes;
-	a->ext_n = n_reads;
 	return ABB_OK;
 }
 

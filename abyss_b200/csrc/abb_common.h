@@ -162,8 +162,16 @@ inline unsigned sm_count()
 	return n > 0 ? (unsigned)n : 132;
 }
 
-// host helpers implemented in abb_api.cu, shared with abb_assemble.cu
+// host helpers implemented in abb_api.cu, shared with the other C-ABI translation units
 int select_device(int device);
+/** A host read batch (bases, offsets[n_reads + 1]) as the C ABI takes it: ABB_EINVAL unless the buffers are given and
+ *  offsets[0] == 0; "NULL <noun> buffers" names them.  Host only, so a malformed batch is refused without a device.
+ *  An empty batch needs no buffers. */
+int check_read_batch(const char* bases, const uint64_t* offsets, uint64_t n_reads, const char* noun = "read");
+/** Queues the copy of a checked host read batch to d_bases (16 bytes of slack) and d_offs on `stream`, growing them as
+ *  needed.  With bases NULL only d_bases is sized: the caller copies the bases itself. */
+int stage_read_batch(const char* bases, const uint64_t* offsets, uint64_t n_reads, DevBuf<uint8_t>& d_bases, DevBuf<uint64_t>& d_offs,
+                     cudaStream_t stream);
 /** slot_offs[0..n_reads] = exclusive prefix sum of per-read k-mer window counts; *total = sum */
 int compute_slot_offsets(unsigned k, const uint64_t* d_offs, uint64_t n_reads, DevBuf<uint64_t>& slot_offs,
                          DevBuf<uint8_t>& tmp, cudaStream_t stream, uint64_t* total, uint64_t* launches);
@@ -172,11 +180,36 @@ int compute_slot_offsets(unsigned k, const uint64_t* d_offs, uint64_t n_reads, D
 
 struct abb_filter;
 namespace abb {
+/** device-resident control block of the ordered insert (abb_insert.cuh) */
+struct InsertCtl {
+	unsigned n_carry[2];  // lengths of the two carry lists
+	unsigned old_flag;    // a slot carried again is older than the drain age
+	unsigned resume;      // first window the kernel has NOT processed (it stops early when a drain is due)
+	unsigned tag_mask[2]; // prefix of each tag table that is in use (to be cleared before its next use)
+};
+struct ShardCtl; // abb_shard.cuh
+
+/** the words of abb_filter::d_stats; no two operations share one.  The first three accumulate over calls
+ *  (abb_filter_insert_stats reads and resets them), each of the others is cleared by the call that uses it. */
+enum StatWord : unsigned {
+	kStatDeferred,                     // slots that did not commit in their own window
+	kStatDrains,                       // drains that did work
+	kStatDrainedSlots,                 // slots replayed by drains
+	kStatInsertKmers,                  // valid k-mers of one insert (k_count_valid)
+	kStatKonKmers,                     // k-mers of one Konnector insert
+	kStatPopcount,                     // [2] abb_filter_popcount: nonzero, at or above the threshold
+	kStatLevelPop = kStatPopcount + 2, // abb_filter_level_popcount
+	kStatCompare,                      // [3] abb_filter_compare: the 1/1, 1/0 and 0/1 bit counts
+	kStatWords = kStatCompare + 3
+};
+
 /** K1 for reads [r0, r1): h0/valid index = slot_offs[r] + j - slot_base */
 int launch_hash(unsigned k, const uint8_t* d_care, const uint8_t* d_bases, const uint64_t* d_offs, const uint64_t* d_slot_offs,
                 uint64_t r0, uint64_t r1, uint64_t slot_base, uint64_t* d_h0, uint8_t* d_valid, cudaStream_t stream, uint64_t* launches);
 int launch_hash_segments(unsigned k, const uint8_t* d_care, const uint8_t* d_bases, const uint64_t* d_seg_beg, const unsigned* d_seg_len,
                          const uint64_t* d_seg_slot, uint64_t n_segs, uint64_t* d_h0, uint8_t* d_valid, cudaStream_t stream);
+/** level -1 is the last one; ABB_EINVAL for a level the filter does not have */
+int resolve_level(const abb_filter* f, int level, unsigned* out);
 // abb_konnector.cu: the ABB_KONNECTOR paths of abb_insert_reads(_dev) and abb_contains_reads
 int kon_insert_reads_dev(abb_filter* f, const uint8_t* d_bases, const uint64_t* d_offs, uint64_t n_reads, uint64_t* n_kmers_out);
 /** membership of the last level and validity of every window slot (f->slot_offs already computed) into f->out8 / f->valid */
@@ -213,8 +246,9 @@ struct abb_filter {
 	abb::DevBuf<uint64_t> d_carry;    // two carry lists and the drain's sorted list, (window + kCarryLanes) slots each
 	abb::DevBuf<unsigned> d_slotbits; // presence bitmap of the drain
 	uint64_t slotbit_words = 0;
-	abb::DevBuf<unsigned> d_ctl;             // abb::InsertCtl
-	abb::DevBuf<unsigned long long> d_stats; // [0] deferred [1] drains [2] slots replayed by drains [3..4] popcount scratch
+	abb::DevBuf<abb::InsertCtl> d_ctl;
+	abb::DevBuf<abb::ShardCtl> d_shard_ctl;
+	abb::DevBuf<unsigned long long> d_stats; // abb::kStatWords words, abb::StatWord
 
 	// per-call buffers (bases/offs keep the device copy of the last host batch: abb_filter_resident_reads)
 	uint64_t resident_reads = 0;
@@ -237,6 +271,8 @@ struct abb_filter {
 	/** device bytes from one level to the next.  Bit and cascading levels start on 16-byte boundaries: bits_set ORs 4-byte words
 	 *  and k_popcount loads uint4, while size / 8 need only be a multiple of 1.  Counting filters have one level, and the
 	 *  Konnector kernels address a packed array of levels.  The padding is never part of a level: bytes_per_level is. */
+	/** bits of one level: a Konnector filter holds `size` bits, the others a whole number of bytes */
+	uint64_t bits_per_level() const { return kind == ABB_KONNECTOR ? size : bytes_per_level * 8; }
 	uint64_t level_stride() const { return kind == ABB_BIT || kind == ABB_CASCADING ? (bytes_per_level + 15) & ~15ULL : bytes_per_level; }
 	uint8_t* level_data(unsigned level) const { return d_data.p + (uint64_t)level * level_stride(); }
 

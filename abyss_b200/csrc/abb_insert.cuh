@@ -34,6 +34,7 @@
 // Tag entries are [position + 1 : 36 | priority : 28], 0 = empty; a window uses only a prefix of
 // the table sized to its carried slots, and that prefix is cleared before the table's next use.
 #pragma once
+#include "abb_common.h"
 #include "abb_device.cuh"
 #include "abb_graph.cuh"
 #include <cooperative_groups.h>
@@ -478,15 +479,6 @@ ABB_D unsigned map_get(const ConflictMap& m, uint64_t pos)
 	return (__ldcg(&m.w[e >> 4]) >> ((unsigned)(e & 15) * 2)) & 3u;
 }
 
-/** device-resident control block of the insert pipeline */
-struct InsertCtl {
-	unsigned n_carry[2];  // lengths of the two carry lists
-	unsigned old_flag;    // a slot carried again is older than the drain age
-	unsigned resume;      // first window the kernel has NOT processed (it stops early when a drain is due)
-	unsigned tag_mask[2]; // prefix of each tag table that is in use (to be cleared before its next use)
-	unsigned pad[2];
-};
-
 /** CountingBloomFilter::incrementMin / HashAgnosticCascadingBloom::insert by a thread that is the
  *  only pending event on all of its positions */
 template <int KIND, int MAXH>
@@ -639,7 +631,7 @@ k_insert_windows(const InsertArgs a)
 					apply_alone<KIND, MAXH>(a.f, pos, v, H);
 				else {
 					a.carry[out][atomicAdd(&a.ctl->n_carry[out], 1u)] = w0 + t;
-					atomicAdd(&a.stats[0], 1ULL); // slots that did not commit in their own window
+					atomicAdd(&a.stats[kStatDeferred], 1ULL);
 				}
 			}
 		}
@@ -745,7 +737,7 @@ ABB_D unsigned enumerate_presence(unsigned* __restrict__ bw, unsigned words, uin
 /** K2c.  Does nothing unless forced, more than min_count slots are pending or a pending slot is old.
  *  Clears ctl->n_carry[other] (the list the preceding window launch has just consumed) so that it can collect
  *  the next window's carries.  `bits` is a zeroed presence bitmap for slots [lo_slot, lo_slot + 32 * bit_words)
- *  (left zeroed), `sorted` holds as many slots as the list.  stats[2] += slots replayed. */
+ *  (left zeroed), `sorted` holds as many slots as the list.  stats[kStatDrainedSlots] += slots replayed. */
 template <int KIND, bool LITERAL, int MAXH>
 __global__ void __launch_bounds__(kDrainThreads)
 k_drain(const uint64_t* __restrict__ hashes, HashCfg cfg, FilterView f, const uint64_t* __restrict__ list, InsertCtl* __restrict__ ctl,
@@ -862,8 +854,8 @@ k_drain(const uint64_t* __restrict__ hashes, HashCfg cfg, FilterView f, const ui
 	if (threadIdx.x == 0) {
 		ctl->n_carry[which] = 0;
 		ctl->old_flag = 0;
-		atomicAdd(&stats[2], (unsigned long long)n);
-		atomicAdd(&stats[1], 1ULL); // drains that did work
+		atomicAdd(&stats[kStatDrainedSlots], (unsigned long long)n);
+		atomicAdd(&stats[kStatDrains], 1ULL);
 	}
 }
 

@@ -38,7 +38,7 @@ int kon_insert_reads_dev(abb_filter* f, const uint8_t* d_bases, const uint64_t* 
 	ABB_CHECK(compute_slot_offsets(f->k, d_offs, n_reads, f->slot_offs, f->scan_tmp, f->stream, &total, &f->st.launches));
 	if (total == 0)
 		return ABB_OK;
-	unsigned long long* d_count = f->d_stats.p + 6;
+	unsigned long long* d_count = f->d_stats.p + kStatKonKmers;
 	ABB_CUDA(cudaMemsetAsync(d_count, 0, sizeof(unsigned long long), f->stream));
 	ABB_CUDA(cudaEventRecord(f->ev0, f->stream));
 	k_kon_walk<false><<<kon_grid(total), 256, 0, f->stream>>>(d_bases, d_offs, f->slot_offs.p, n_reads, total, kon_geom(f->k), kon_view(f),
@@ -77,10 +77,9 @@ int abb_filter_read_bits(abb_filter* f, int level, const uint8_t* host, uint64_t
 	ABB_REQUIRE(f, "NULL filter");
 	ABB_REQUIRE(f->kind != ABB_COUNTING, "readBits applies to bit filters");
 	ABB_REQUIRE(op == KON_OVERWRITE || op == KON_OR || op == KON_AND, "op must be 0 (overwrite), 1 (or) or 2 (and)");
-	if (level < 0)
-		level = (int)f->levels - 1;
-	ABB_REQUIRE((unsigned)level < f->levels, "level %d out of range", level);
-	const uint64_t size = f->kind == ABB_KONNECTOR ? f->size : f->bytes_per_level * 8;
+	unsigned l = 0;
+	ABB_CHECK(resolve_level(f, level, &l));
+	const uint64_t size = f->bits_per_level();
 	ABB_REQUIRE(bit_offset <= size && bits <= size - bit_offset, "%llu bits at bit %llu do not fit in %llu bits", (unsigned long long)bits,
 	            (unsigned long long)bit_offset, (unsigned long long)size);
 	if (bits == 0)
@@ -93,7 +92,7 @@ int abb_filter_read_bits(abb_filter* f, int level, const uint8_t* host, uint64_t
 	ABB_CUDA(cudaMemcpyAsync(src.p, host, nbytes, cudaMemcpyHostToDevice, f->stream));
 	const uint64_t dest_bytes = bit_offset / 8 + nbytes + 1;
 	k_kon_read_bits<<<std::min<unsigned>(blocks_for(dest_bytes, 256), sm_count() * 16), 256, 0, f->stream>>>(
-	    f->level_data((unsigned)level), f->bytes_per_level, src.p, bits, bit_offset, op);
+	    f->level_data(l), f->bytes_per_level, src.p, bits, bit_offset, op);
 	f->st.launches += 1;
 	ABB_CUDA(cudaGetLastError());
 	ABB_CUDA(cudaStreamSynchronize(f->stream));
@@ -104,13 +103,12 @@ int abb_filter_level_popcount(abb_filter* f, int level, uint64_t* n)
 {
 	ABB_REQUIRE(f && n, "NULL argument");
 	ABB_REQUIRE(f->kind != ABB_COUNTING, "the level population applies to bit filters");
-	if (level < 0)
-		level = (int)f->levels - 1;
-	ABB_REQUIRE((unsigned)level < f->levels, "level %d out of range", level);
+	unsigned l = 0;
+	ABB_CHECK(resolve_level(f, level, &l));
 	ABB_CUDA(cudaSetDevice(f->device));
-	unsigned long long* d_n = f->d_stats.p + 6;
+	unsigned long long* d_n = f->d_stats.p + kStatLevelPop;
 	ABB_CUDA(cudaMemsetAsync(d_n, 0, sizeof(unsigned long long), f->stream));
-	k_kon_popcount<<<sm_count() * 8, 256, 0, f->stream>>>(f->level_data((unsigned)level), f->bytes_per_level, d_n);
+	k_kon_popcount<<<sm_count() * 8, 256, 0, f->stream>>>(f->level_data(l), f->bytes_per_level, d_n);
 	f->st.launches += 1;
 	ABB_CUDA(cudaGetLastError());
 	unsigned long long h = 0;
@@ -130,13 +128,12 @@ int abb_trim_reads(abb_filter* f, const char* bases, const uint64_t* offsets, ui
 	}
 	if (n_reads == 0)
 		return ABB_OK;
-	ABB_REQUIRE(bases && offsets && left && right, "NULL buffer");
-	ABB_REQUIRE(offsets[0] == 0, "offsets[0] must be 0");
+	ABB_REQUIRE(left && right, "NULL buffer");
+	ABB_CHECK(check_read_batch(bases, offsets, n_reads));
 	ABB_REQUIRE(f->k >= 2, "k must be at least 2");
 	for (uint64_t r = 0; r < n_reads; ++r)
 		ABB_REQUIRE(offsets[r + 1] - offsets[r] < (1ULL << 31), "read %llu is too long", (unsigned long long)r);
 	ABB_CUDA(cudaSetDevice(f->device));
-	const uint64_t n_bases = offsets[n_reads];
 	int per_sm = 0; // a grid that is resident all at once: the walk scratch is sized per warp of the grid
 	ABB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_kon_trim, kKonTrimThreads, 0));
 	const unsigned blocks =
@@ -146,15 +143,12 @@ int abb_trim_reads(abb_filter* f, const char* bases, const uint64_t* offsets, ui
 	DevBuf<uint64_t>& d_offs = f->trim_offs;
 	DevBuf<uint32_t>& d_out = f->trim_out;
 	const size_t frame_bytes = n_warps * kFrameCap * sizeof(Frame);
-	ABB_CHECK(d_bases.reserve(n_bases + 16));
-	ABB_CHECK(d_offs.reserve(n_reads + 1));
 	ABB_CHECK(f->trim_scratch.reserve(frame_bytes + n_warps * kLookCap * sizeof(uint64_t)));
 	ABB_CHECK(d_out.reserve(2 * n_reads));
 	Frame* d_frames = reinterpret_cast<Frame*>(f->trim_scratch.p);
 	uint64_t* d_look = reinterpret_cast<uint64_t*>(f->trim_scratch.p + frame_bytes);
 	const SyncOnExit sync = { f->stream };
-	ABB_CUDA(cudaMemcpyAsync(d_bases.p, bases, n_bases, cudaMemcpyHostToDevice, f->stream));
-	ABB_CUDA(cudaMemcpyAsync(d_offs.p, offsets, (n_reads + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, f->stream));
+	ABB_CHECK(stage_read_batch(bases, offsets, n_reads, d_bases, d_offs, f->stream));
 	k_kon_trim<<<blocks, kKonTrimThreads, 0, f->stream>>>(d_bases.p, d_offs.p, n_reads, kon_geom(f->k), kon_view(f), min_branch_len, d_frames,
 	                                                      d_look, d_out.p, d_out.p + n_reads);
 	ABB_CUDA(cudaGetLastError());
@@ -175,13 +169,12 @@ int abb_filter_compare(abb_filter* a, abb_filter* b, uint64_t counts[4])
 {
 	ABB_REQUIRE(a && b && counts, "NULL argument");
 	ABB_REQUIRE(a->kind != ABB_COUNTING && b->kind != ABB_COUNTING, "compare applies to bit filters");
-	const uint64_t bits_a = a->kind == ABB_KONNECTOR ? a->size : a->bytes_per_level * 8;
-	const uint64_t bits_b = b->kind == ABB_KONNECTOR ? b->size : b->bytes_per_level * 8;
-	ABB_REQUIRE(bits_a == bits_b, "Bit sizes of arrays not equal");
+	const uint64_t bits_a = a->bits_per_level();
+	ABB_REQUIRE(bits_a == b->bits_per_level(), "Bit sizes of arrays not equal");
 	ABB_REQUIRE(a->device == b->device, "the two filters are on different devices");
 	ABB_CUDA(cudaSetDevice(a->device));
 	ABB_CUDA(cudaStreamSynchronize(b->stream));
-	unsigned long long* d_c = a->d_stats.p + 5; // [5..7]
+	unsigned long long* d_c = a->d_stats.p + kStatCompare;
 	ABB_CUDA(cudaMemsetAsync(d_c, 0, 3 * sizeof(unsigned long long), a->stream));
 	const uint64_t nbytes = a->bytes_per_level;
 	k_kon_compare<<<std::min<unsigned>(blocks_for(nbytes, 256), sm_count() * 8), 256, 0, a->stream>>>(

@@ -134,12 +134,9 @@ static int overlap_build(abb_overlap* h, const char* bases, const uint64_t* offs
 	h->st.vertices = 2 * n;
 	if (n == 0)
 		return ABB_OK;
-	const uint64_t n2 = 2 * n, n_bases = offsets[n];
+	const uint64_t n2 = 2 * n;
 	const unsigned k1 = k - 1;
-	ABB_CHECK(h->bases.reserve(n_bases + 16));
-	ABB_CHECK(h->offs.reserve(n + 1));
-	ABB_CUDA(cudaMemcpyAsync(h->bases.p, bases, n_bases, cudaMemcpyHostToDevice, st));
-	ABB_CUDA(cudaMemcpyAsync(h->offs.p, offsets, (n + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
+	ABB_CHECK(stage_read_batch(bases, offsets, n, h->bases, h->offs, st));
 	ABB_CUDA(cudaMemsetAsync(h->d_bad.p, 0, 2 * sizeof(unsigned), st));
 	OvlSeqs s = { h->bases.p, h->offs.p, n, k1 };
 	k_ovl_check_len<<<ovl_grid(n), 256, 0, st>>>(s, h->d_bad.p);
@@ -273,9 +270,8 @@ int abb_overlap_build(abb_overlap* h, const char* bases, const uint64_t* offsets
 	if (n_edges)
 		*n_edges = 0;
 	ABB_REQUIRE(k >= 2, "k must be at least 2");
-	ABB_REQUIRE(n_contigs == 0 || (bases && offsets), "NULL contig buffers");
+	ABB_CHECK(check_read_batch(bases, offsets, n_contigs, "contig"));
 	ABB_REQUIRE(n_contigs < (1ULL << 31), "too many contigs");
-	ABB_REQUIRE(n_contigs == 0 || offsets[0] == 0, "offsets[0] must be 0");
 	// AdjList.cpp:386-388: 0 means k-1, never more than k-1
 	if (min_overlap == 0 || min_overlap > k - 1)
 		min_overlap = k - 1;

@@ -30,7 +30,7 @@ struct Shard {
 /** control block of the sharded pipeline (device) */
 struct ShardCtl {
 	unsigned n_pending;          // slots vetoed in this window/iteration
-	unsigned pad;
+	unsigned n_out;              // length of the carry list k_sh_compact wrote
 	unsigned long long lo_pending; // smallest pending slot (bitmap enumeration starts there)
 };
 
@@ -153,7 +153,7 @@ k_sh_apply(const uint64_t* __restrict__ hashes, const uint8_t* __restrict__ vali
 		atomicAdd(&ctl->n_pending, 1u);
 		atomicMin(&ctl->lo_pending, (unsigned long long)s);
 		if (!carried)
-			atomicAdd(&stats[0], 1ULL);
+			atomicAdd(&stats[kStatDeferred], 1ULL);
 		return;
 	}
 	uint64_t pos[MAXH];

@@ -135,20 +135,18 @@ int abb_mincount_hashes(abb_filter* f, const uint64_t* hashes, uint64_t n, uint8
  * For each read r and window position p < max(0, len_r - k + 1), slot = slot_offsets[r] + p where
  * slot_offsets is the exclusive prefix sum of the per-read window counts.  out_h0[slot] is the
  * canonical (masked) ntHash, out_valid[slot] is 1 if the reference iterator would yield it.
- * Returns the total number of slots through n_slots_out. */
+ * Returns the total number of slots through n_slots_out.  bases / offsets as for abb_insert_reads: a batch whose
+ * offsets[0] is not 0 is refused (ABB_EINVAL), as by every entry point that takes a host read batch. */
 int abb_hash_reads(unsigned k, const char* mask, const char* bases, const uint64_t* offsets,
                    uint64_t n_reads, uint64_t* out_h0, uint8_t* out_valid, uint64_t* n_slots_out,
                    int device);
 
 /* ---- multi-GPU building blocks (SURVEY.md section 8e: hash-range sharding) ------------------
  * abb_hash_reads_dev: K1 only, device in / device out (d_h0, d_valid hold `capacity` slots).
- * abb_insert_h0_dev:  ordered insert of n canonical hashes (device resident, all valid), in array
- *                     order -- what a rank does with the k-mers it owns after the all-to-all.
  * abb_filter_device_ptr: the raw device array of a level, for the NCCL union (all-reduce max /
  *                     or) issued by the caller; synchronises the filter's stream first. */
 int abb_hash_reads_dev(abb_filter* f, const char* d_bases, const uint64_t* d_offsets, uint64_t n_reads,
                        uint64_t* d_h0, uint8_t* d_valid, uint64_t capacity, uint64_t* n_slots_out);
-int abb_insert_h0_dev(abb_filter* f, const uint64_t* d_h0, uint64_t n);
 
 /* ---- multi-GPU exact insert (SURVEY.md section 8e; Bloom/bloom.cc:556-580 `-w M/N` windows are the precedent) -----
  * One process (or host thread) per GPU.  The counter array is sharded by POSITION RANGE: rank r owns counters
@@ -163,7 +161,7 @@ int abb_insert_h0_dev(abb_filter* f, const uint64_t* d_h0, uint64_t n);
  * abb_insert_reads_sharded_dev: EVERY rank passes the same reads (device resident).  finalize != 0 all-gathers the
  *                     shards afterwards so that each rank holds the whole filter (what the extension stage needs);
  *                     with finalize == 0 only the own range of f is meaningful until abb_filter_allgather.
- * abb_comm_allgather_bytes / abb_comm_allreduce_max_u8: the collectives pass 2 needs (read codes, tile stores). */
+ * abb_comm_allgather_bytes / abb_comm_exchange_bytes: the collectives pass 2 needs (read codes, tile stores). */
 typedef struct abb_comm abb_comm;
 int abb_comm_unique_id(uint8_t id_out[128]);
 int abb_comm_create(abb_comm** out, int rank, int world, const uint8_t id[128], int device);
@@ -181,7 +179,6 @@ int abb_filter_allgather(abb_filter* f, abb_comm* c);
 int abb_filter_resident_reads(abb_filter* f, const char** d_bases, const uint64_t** d_offsets, uint64_t* n_reads);
 /* d_buf holds world * bytes_per_rank bytes, this rank's part already in place at rank * bytes_per_rank */
 int abb_comm_allgather_bytes(abb_comm* c, void* d_buf, uint64_t bytes_per_rank, void* cuda_stream);
-int abb_comm_allreduce_max_u8(abb_comm* c, void* d_buf, uint64_t n, void* cuda_stream);
 /* all-gather of unequal parts: this rank's send_bytes go to every other rank; rank r's recv_bytes[r] bytes land at
  * d_recv_base + recv_offsets[r] (grouped ncclSend / ncclRecv; entries for the own rank are ignored) */
 int abb_comm_exchange_bytes(abb_comm* c, const void* d_send, uint64_t send_bytes, void* d_recv_base, const uint64_t* recv_offsets,
@@ -240,13 +237,6 @@ int abb_assembler_process_reads(abb_assembler* a, const char* bases, const uint6
 int abb_assembler_process_reads_dev(abb_assembler* a, const char* d_bases, const uint64_t* d_offsets,
                                     uint64_t n_reads, const abb_contig** contigs, uint64_t* n_contigs,
                                     const char** seqs);
-/* Several GPUs: the per-read classification (K3a) is a pure function of the read and the solid filter, so
- * ranks may classify disjoint slices (abb_assembler_classify_dev writes one code per read, the internal
- * RC_* values, to a device buffer), exchange the codes, and hand the complete array to the rank that
- * assembles: abb_assembler_set_codes applies to the next process_reads call only. */
-int abb_assembler_classify_dev(abb_assembler* a, const char* d_bases, const uint64_t* d_offsets, uint64_t n_reads,
-                               uint8_t* d_codes);
-int abb_assembler_set_codes(abb_assembler* a, const uint8_t* d_codes, uint64_t n_reads);
 /* Start a new assembly on the same handle (the solid filter has been refilled): clears the assembled
  * filter, the contig-end table, the tile store, counters and statistics, keeps all device buffers. */
 int abb_assembler_reset(abb_assembler* a);

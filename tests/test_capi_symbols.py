@@ -45,6 +45,25 @@ def test_no_cpu_fallback(abb):
         raise AssertionError("hash_reads must fail without a CUDA device")
 
 
+def test_hash_reads_refuses_malformed_batch(abb):
+    # the read batch is checked on the host before any CUDA call, so a malformed one is ABB_EINVAL with or without a device
+    import ctypes as C
+    lib = abb.load()
+    bases = np.frombuffer(b"ACGTACGTAC", dtype=np.uint8).copy()
+    offs, shifted = np.array([0, 10], dtype=np.uint64), np.array([1, 10], dtype=np.uint64)
+    h0, valid, n = np.zeros(16, dtype=np.uint64), np.zeros(16, dtype=np.uint8), C.c_uint64(7)
+
+    def run(b, o):
+        return lib.abb_hash_reads(5, b"", b, o, 1, h0.ctypes.data, valid.ctypes.data, C.byref(n), 0)
+
+    assert run(None, offs.ctypes.data) == abb.ABB_EINVAL
+    assert "NULL read buffers" in lib.abb_last_error().decode()
+    assert run(bases.ctypes.data, None) == abb.ABB_EINVAL
+    assert run(bases.ctypes.data, shifted.ctypes.data) == abb.ABB_EINVAL
+    assert "offsets[0] must be 0" in lib.abb_last_error().decode()
+    assert n.value == 0
+
+
 def test_header_is_plain_c(tmp_path):
     # the boundary is a C ABI: include/abyss_b200.h compiles as C99 (no C++, no torch or CUDA types) and a C program links against
     # the library using nothing but that header

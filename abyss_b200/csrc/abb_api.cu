@@ -25,7 +25,6 @@ void set_error(const char* fmt, ...)
 	va_end(ap);
 }
 
-constexpr uint64_t kDefaultWindow = 1ULL << 17;
 constexpr uint64_t kChunkSlots = 1ULL << 27; // h0 staging: 128 Mi slots = 1 GiB + 128 MiB flags (one persistent launch + one forced drain per chunk)
 
 static uint64_t next_pow2(uint64_t x)
@@ -63,18 +62,31 @@ static FilterView view_of(const abb_filter* f)
 }
 
 /** conflict-map size: 2^25 two-bit entries (8 MiB per map; the three rotating maps are pinned in L2 while the insert
- *  runs, set_l2_policy); with the default window of 2^17 slots 6.4 % of the slots see an alias and are carried (2^26
- *  halves that and measured 3 % slower: the maps compete with the counter sectors for L2).  Exact (no aliases) for
- *  filters of up to 2^25 positions. */
+ *  runs, set_l2_policy), split into the two halves of 2^24 entries of a two-index map (ConflictMap2, abb_insert.cuh).
+ *  Exact (no aliases) for filters of up to 2^24 positions. */
 constexpr unsigned kMapLog2 = 25;
-/** the sharded insert's maps: each rank marks window * H / world positions, 2^20 at the default window */
+static_assert(kMapLog2 - 1 <= kMapHalfLog2Max, "half B of a conflict map cannot index more than 2^24 entries");
+/** ordered-insert window (slots) when none was set.  A filter with more positions than a map half has entries aliases in
+ *  the maps; there the two-index maps carry 1.7 % of the slots at 2^18 slots per window (bench job; one map of 2^25
+ *  entries carried 6.4 % at 2^17), and the larger window halves the fixed cost per slot of the windows (two grid
+ *  barriers, a map clear and the carried slots' reservations each).  2^19 carried 6.4 % again and measured slower (DESIGN
+ *  §3 K2).  A filter the maps cover exactly has no false carries, only true ones, which grow with the window: it keeps
+ *  2^17. */
+constexpr uint64_t kDefaultWindow = 1ULL << 18;
+constexpr uint64_t kExactMapWindow = 1ULL << 17;
+static uint64_t default_window(uint64_t filter_size)
+{
+	return filter_size > (1ULL << (kMapLog2 - 1)) ? kDefaultWindow : kExactMapWindow;
+}
+/** the sharded insert's maps (one index): each rank marks window * H / world positions */
 constexpr unsigned kShardMapLog2 = 27;
 
-/** entries per conflict map: 2^lg, or fewer when the filter has fewer positions */
-static uint64_t map_entries_for(uint64_t filter_size, unsigned lg)
+/** entries per conflict map of `halves` equal parts: 2^lg in all, or fewer when the filter has fewer positions (each part
+ *  then still has an entry per position) */
+static uint64_t map_entries_for(uint64_t filter_size, unsigned lg, unsigned halves)
 {
 	const uint64_t fit = std::max<uint64_t>(next_pow2(filter_size), 1024);
-	return std::min<uint64_t>(1ULL << lg, fit);
+	return halves * std::min<uint64_t>((1ULL << lg) / halves, fit);
 }
 
 static unsigned age_windows_for(uint64_t window)
@@ -83,10 +95,10 @@ static unsigned age_windows_for(uint64_t window)
 }
 
 /** make sure the ordered-insert workspace exists for `window` slots per window, conflict maps of 2^lg entries (at
- *  most) and the current hash count */
-static int ensure_workspace(abb_filter* f, uint64_t window, unsigned lg)
+ *  most) in `halves` parts and the current hash count */
+static int ensure_workspace(abb_filter* f, uint64_t window, unsigned lg, unsigned halves)
 {
-	const uint64_t want_entries = map_entries_for(f->size, lg);
+	const uint64_t want_entries = map_entries_for(f->size, lg, halves);
 	if (f->d_carry.p && f->ws_window == window && f->ws_H == f->H && f->map_entries == want_entries)
 		return ABB_OK;
 	// the old workspace is freed before the new one is allocated (peak memory), and it counts as valid again only once
@@ -242,7 +254,7 @@ static int ordered_insert(abb_filter* f, const uint64_t* d_hashes, const uint8_t
 		ABB_CUDA(cudaGetLastError());
 		return ABB_OK;
 	}
-	ABB_CHECK(ensure_workspace(f, f->window, kMapLog2));
+	ABB_CHECK(ensure_workspace(f, f->window, kMapLog2, 2));
 	cudaStream_t st = f->stream;
 	const uint64_t W = f->window;
 	const uint64_t n_windows = (n_slots + W - 1) / W;
@@ -256,10 +268,8 @@ static int ordered_insert(abb_filter* f, const uint64_t* d_hashes, const uint8_t
 	a.w_begin = 0;
 	a.n_windows = (unsigned)n_windows;
 	a.cfg = f->cfg;
-	for (int i = 0; i < 3; ++i) {
-		a.map[i].w = f->d_map[i];
-		a.map[i].mask = f->map_entries - 1;
-	}
+	for (int i = 0; i < 3; ++i)
+		a.map[i].a = { f->d_map[i], f->map_entries / 2 - 1 }; // half B follows half A
 	for (int i = 0; i < 2; ++i) {
 		a.tags[i] = f->d_tags2[i].p;
 		a.carry[i] = f->d_carry.p + (uint64_t)i * cap;
@@ -634,11 +644,13 @@ namespace abb {
 
 static uint64_t shard_chunk(uint64_t size, unsigned world) { return ((size + world - 1) / world + 15) & ~15ULL; }
 
-/** the window of the sharded pipeline: per-rank conflict-map load like the single-GPU window */
+/** the window of the sharded pipeline: 2^18 slots per rank by default (twice the per-rank load of its one-index conflict
+ *  maps at 2^17 slots), twice the filter's window per rank when one was set */
+constexpr uint64_t kShardRankWindow = 1ULL << 18;
 static uint64_t sharded_window(const abb_filter* f, unsigned world)
 {
-	const uint64_t w = 2 * f->window * world; // 2^18 slots per rank: the per-rank conflict-map load of the single-GPU window, twice
-	return std::min<uint64_t>(std::max<uint64_t>(w, 32), 1ULL << 21);
+	const uint64_t per_rank = f->window == default_window(f->size) ? kShardRankWindow : 2 * f->window;
+	return std::min<uint64_t>(std::max<uint64_t>(per_rank * world, 32), 1ULL << 21);
 }
 
 static int sharded_ordered_insert(abb_filter* f, abb_comm* c, const uint64_t* d_h0, const uint8_t* d_valid, uint64_t n_slots)
@@ -646,7 +658,7 @@ static int sharded_ordered_insert(abb_filter* f, abb_comm* c, const uint64_t* d_
 	if (n_slots == 0)
 		return ABB_OK;
 	const uint64_t W = sharded_window(f, (unsigned)c->world);
-	ABB_CHECK(ensure_workspace(f, W, kShardMapLog2));
+	ABB_CHECK(ensure_workspace(f, W, kShardMapLog2, 1));
 	// carried slots served per step: the tag table holds only own positions, so world times the single-GPU number fit
 	const unsigned max_lanes = (unsigned)std::min<uint64_t>((uint64_t)kCarryLanes * (unsigned)c->world, W / 2 + kCarryLanes);
 	ABB_CHECK(f->sh_buf.reserve(2 * (W + (uint64_t)max_lanes) + 64));
@@ -828,7 +840,7 @@ int abb_filter_create(abb_filter** out, int kind, uint64_t size, unsigned num_ha
 	f->threshold = kind == ABB_COUNTING ? arg : 0;
 	f->levels = levels;
 	f->mask = m;
-	f->window = kDefaultWindow;
+	f->window = default_window(size);
 	f->cfg.H = num_hashes;
 	f->cfg.k = k;
 	f->cfg.mod = make_fastmod(size);
@@ -940,7 +952,7 @@ int abb_filter_set_window(abb_filter* f, uint64_t window_slots)
 {
 	ABB_REQUIRE(f, "NULL filter");
 	if (window_slots == 0)
-		window_slots = kDefaultWindow;
+		window_slots = default_window(f->size);
 	ABB_REQUIRE(window_slots >= 32 && window_slots <= (1ULL << 20) - 64, "window must be in [32, 2^20 - 64]");
 	ABB_CUDA(cudaSetDevice(f->device));
 	ABB_CUDA(cudaStreamSynchronize(f->stream));
@@ -984,7 +996,7 @@ int abb_insert_reads(abb_filter* f, const char* bases, const uint64_t* offsets, 
 	if (!f->copy_stream)
 		ABB_CUDA(cudaStreamCreateWithFlags(f->copy_stream.out(), cudaStreamNonBlocking));
 	if (f->kind != ABB_BIT)
-		ABB_CHECK(ensure_workspace(f, f->window, kMapLog2)); // the maps exist before the policy that pins them is set
+		ABB_CHECK(ensure_workspace(f, f->window, kMapLog2, 2)); // the maps exist before the policy that pins them is set
 	PolicyHold policy(f, 3); // before the copy starts: setting it later would wait for the whole copy (see PolicyHold)
 	PendingCopy pc;
 	pc.h_offs = offsets;

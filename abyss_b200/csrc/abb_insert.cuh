@@ -14,11 +14,13 @@
 //   * k-mer windows ("slots") are numbered in file order; a batch is cut into ordered windows of
 //     W slots; windows run one after another, slots inside a window run in parallel.
 //   * conflict map: every slot of window w marks its H filter positions in an L2-resident map of
-//     two-bit entries (entry = position mod E): "touched" / "touched again".  A slot none of whose
-//     entries was touched again shares no counter with any other pending event: it commutes with
-//     all of them, so it applies its min-increment at once with plain byte loads/stores.  That is
-//     ~97 % of the slots and costs one L2 atomic + one L2 load per position on top of the HBM
-//     accesses themselves (round 1: CAS + probe + release on an 8-byte tag per position).
+//     two-bit entries: "touched" / "touched again".  The map has two halves indexed two ways
+//     (position mod E, and a hash of the position; ConflictMap2), and an entry counts as touched
+//     again only if both halves say so.  A slot none of whose entries was touched again shares no
+//     counter with any other pending event: it commutes with all of them, so it applies its
+//     min-increment at once with plain byte loads/stores.  That is ~98 % of the slots and costs two
+//     L2 atomics + two L2 loads per position on top of the HBM accesses themselves (round 1: CAS +
+//     probe + release on an 8-byte tag per position).
 //     The marks of window w+1 are written by the kernel that applies window w.
 //   * carry: the slots that saw "touched again" (true sharing, or an alias in the map) are carried
 //     into the next window as its OLDEST events.  Carried slots are few, so they use an exact
@@ -432,51 +434,91 @@ ABB_D uint64_t slot_position(const uint64_t* __restrict__ hashes, uint64_t s, co
 	return LITERAL ? fastmod_u64(hashes[s * cfg.H + i], cfg.mod) : nth_pos(hashes[s], cfg, i);
 }
 
-/** conflict map: E two-bit entries, 16 per word, entry = position mod E (E a power of two; exact when the
- *  filter has at most E positions).  bit 0: touched by a slot of the window; bit 1: touched again (by a second
- *  slot, by a second hash of the same slot, or by a carried slot). */
+/** conflict map: E two-bit entries, 16 per word, entry = key mod E (E a power of two; exact when the keys are
+ *  positions and the filter has at most E of them).  bit 0: touched by a slot of the window; bit 1: touched again (by a
+ *  second slot, by a second hash of the same slot, or by a carried slot). */
 struct ConflictMap {
 	unsigned* w;
 	uint64_t mask; // E - 1
 };
-ABB_D void map_mark(const ConflictMap& m, uint64_t pos)
+/** first half of a mark: "touched"; returns the entry's word as it was */
+ABB_D unsigned map_touch(const ConflictMap& m, uint64_t key)
 {
-	const uint64_t e = pos & m.mask;
+	const uint64_t e = key & m.mask;
+	return atomicOr(&m.w[e >> 4], 1u << ((unsigned)(e & 15) * 2));
+}
+/** second half: "touched again" if the word map_touch returned says the entry was touched already */
+ABB_D void map_touch_again(const ConflictMap& m, uint64_t key, unsigned old)
+{
+	const uint64_t e = key & m.mask;
 	const unsigned sh = (unsigned)(e & 15) * 2;
-	const unsigned old = atomicOr(&m.w[e >> 4], 1u << sh);
 	if (((old >> sh) & 3u) == 1u)
 		atomicOr(&m.w[e >> 4], 2u << sh);
 }
-/** the marks of all H positions of a slot: the H first atomics are independent and in flight together; only then are
- *  their return values looked at (a mark issued per position would serialise H L2 round trips per thread) */
-template <int MAXH>
-ABB_D void map_mark_all(const ConflictMap& m, const uint64_t* pos, unsigned H)
+ABB_D void map_mark_carried(const ConflictMap& m, uint64_t key)
 {
-	unsigned old[MAXH];
-#pragma unroll
-	for (int i = 0; i < MAXH; ++i)
-		if (i < (int)H) {
-			const uint64_t e = pos[i] & m.mask;
-			old[i] = atomicOr(&m.w[e >> 4], 1u << ((unsigned)(e & 15) * 2));
-		}
-#pragma unroll
-	for (int i = 0; i < MAXH; ++i)
-		if (i < (int)H) {
-			const uint64_t e = pos[i] & m.mask;
-			const unsigned sh = (unsigned)(e & 15) * 2;
-			if (((old[i] >> sh) & 3u) == 1u)
-				atomicOr(&m.w[e >> 4], 2u << sh);
-		}
-}
-ABB_D void map_mark_carried(const ConflictMap& m, uint64_t pos)
-{
-	const uint64_t e = pos & m.mask;
+	const uint64_t e = key & m.mask;
 	atomicOr(&m.w[e >> 4], 3u << ((unsigned)(e & 15) * 2));
 }
-ABB_D unsigned map_get(const ConflictMap& m, uint64_t pos)
+ABB_D unsigned map_get(const ConflictMap& m, uint64_t key)
 {
-	const uint64_t e = pos & m.mask;
+	const uint64_t e = key & m.mask;
 	return (__ldcg(&m.w[e >> 4]) >> ((unsigned)(e & 15) * 2)) & 3u;
+}
+/** zero the map; called by every thread of the grid (T threads, this one gtid) */
+ABB_D void map_clear(const ConflictMap& m, uint64_t gtid, uint64_t T)
+{
+	uint4* mw = reinterpret_cast<uint4*>(m.w);
+	const uint64_t words4 = (m.mask + 1) / 64; // 16 entries per word, 4 words per uint4
+	for (uint64_t i = gtid; i < words4; i += T)
+		mw[i] = make_uint4(0, 0, 0, 0);
+}
+
+/** the ordered insert's two-index conflict map: two single maps ("halves") of E entries each, every mark goes into both.
+ *  Half A is indexed by the position mod E, half B by a multiplicative hash of the whole position, and a position counts
+ *  as touched again only if both halves say so.  Two positions that share their half-A entry (they differ by a multiple
+ *  of E) rarely share their half-B entry too, so a window of W slots sees about q^2 false alarms per position instead of
+ *  q = 1 - exp(-W H / E) -- at the same L2 footprint as one map of 2E entries.  Still conservative: a true second event on
+ *  a position sets "touched again" at its entry in both halves.  When the filter has at most E positions half A alone is
+ *  exact, and the AND keeps it so. */
+struct ConflictMap2 {
+	ConflictMap a; // half A; half B is the E entries that follow it (one pointer and one mask: the kernel keeps two maps in registers)
+	ABB_D ConflictMap b() const { return { a.w + (a.mask + 1) / 16, a.mask }; } // 16 entries per word
+};
+constexpr unsigned kMapHalfLog2Max = 24; // half B takes its index from the top 24 bits of a 64-bit product
+ABB_D uint64_t map_key_b(uint64_t pos) { return (pos * 0xD6E8FEB86659FD93ULL) >> (64 - kMapHalfLog2Max); }
+/** the marks of all H positions of a slot: the 2H first atomics are independent and in flight together; only then are
+ *  their return values looked at (a mark issued per position would serialise H L2 round trips per thread) */
+template <int MAXH>
+ABB_D void map_mark_all(const ConflictMap2& m, const uint64_t* pos, unsigned H)
+{
+	unsigned old_a[MAXH], old_b[MAXH];
+#pragma unroll
+	for (int i = 0; i < MAXH; ++i)
+		if (i < (int)H) {
+			old_a[i] = map_touch(m.a, pos[i]);
+			old_b[i] = map_touch(m.b(), map_key_b(pos[i]));
+		}
+#pragma unroll
+	for (int i = 0; i < MAXH; ++i)
+		if (i < (int)H) {
+			map_touch_again(m.a, pos[i], old_a[i]);
+			map_touch_again(m.b(), map_key_b(pos[i]), old_b[i]);
+		}
+}
+ABB_D void map_mark_carried(const ConflictMap2& m, uint64_t pos)
+{
+	map_mark_carried(m.a, pos);
+	map_mark_carried(m.b(), map_key_b(pos));
+}
+ABB_D unsigned map_get(const ConflictMap2& m, uint64_t pos)
+{
+	return map_get(m.a, pos) & map_get(m.b(), map_key_b(pos));
+}
+ABB_D void map_clear(const ConflictMap2& m, uint64_t gtid, uint64_t T)
+{
+	map_clear(m.a, gtid, T);
+	map_clear(m.b(), gtid, T);
 }
 
 /** CountingBloomFilter::incrementMin / HashAgnosticCascadingBloom::insert by a thread that is the
@@ -508,7 +550,7 @@ struct InsertArgs {
 	unsigned window;        // W
 	unsigned w_begin, n_windows;
 	HashCfg cfg;
-	ConflictMap map[3];     // window w reads map[w % 3], marks map[(w+1) % 3] and clears map[(w+2) % 3] (read by window w-1)
+	ConflictMap2 map[3];    // window w reads map[w % 3], marks map[(w+1) % 3] and clears map[(w+2) % 3] (read by window w-1)
 	unsigned long long* tags[2];
 	unsigned tag_cap;       // entries allocated per tag table (power of two)
 	FilterView f;
@@ -558,9 +600,9 @@ k_insert_windows(const InsertArgs a)
 	}
 	for (unsigned w = a.w_begin; w < a.n_windows; ++w) {
 		const int in = (int)(w & 1), out = 1 - in;
-		const ConflictMap& mcur = a.map[w % 3];
-		const ConflictMap& mnext = a.map[(w + 1) % 3];
-		const ConflictMap& mold = a.map[(w + 2) % 3];
+		const ConflictMap2& mcur = a.map[w % 3];
+		const ConflictMap2& mnext = a.map[(w + 1) % 3];
+		const ConflictMap2& mold = a.map[(w + 2) % 3];
 		const uint64_t w0 = (uint64_t)w * W, w1 = w0 + W;
 		const unsigned n = (unsigned)min(W, a.n_slots - w0);
 		const unsigned n_next = w + 1 < a.n_windows ? (unsigned)min(W, a.n_slots - w1) : 0u;
@@ -637,10 +679,7 @@ k_insert_windows(const InsertArgs a)
 		}
 		for (uint64_t i = gtid; i <= old_mask_out; i += T) // the tag table of window w - 1
 			a.tags[out][i] = 0;
-		uint4* mw = reinterpret_cast<uint4*>(mold.w); // ... and its conflict map
-		const uint64_t words4 = (mold.mask + 1) / 64; // 16 entries per word, 4 words per uint4
-		for (uint64_t i = gtid; i < words4; i += T)
-			mw[i] = make_uint4(0, 0, 0, 0);
+		map_clear(mold, gtid, T); // ... and its conflict map
 		grid.sync(); // (a grid barrier orders memory itself)
 		// ---- phase B
 		const unsigned n_out = a.ctl->n_carry[out];

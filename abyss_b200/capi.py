@@ -51,7 +51,8 @@ class AssemblyStats(C.Structure):
     _fields_ = [("rounds", C.c_uint64), ("speculated_reads", C.c_uint64), ("wasted_reads", C.c_uint64),
                 ("candidates", C.c_uint64), ("contigs_tried", C.c_uint64), ("launches", C.c_uint64),
                 ("ms_classify", C.c_float), ("ms_visited", C.c_float), ("ms_extend", C.c_float), ("ms_replay", C.c_float),
-                ("ms_tiles", C.c_float), ("ms_walk", C.c_float), ("ms_stage", C.c_float), ("ms_repeat", C.c_float), ("ms_total", C.c_float), ("ms_cand", C.c_float), ("markers", C.c_uint64), ("tiles", C.c_uint64), ("serial_fallbacks", C.c_uint64)]
+                ("ms_tiles", C.c_float), ("ms_walk", C.c_float), ("ms_stage", C.c_float), ("ms_repeat", C.c_float), ("ms_total", C.c_float), ("ms_cand", C.c_float), ("markers", C.c_uint64), ("tiles", C.c_uint64), ("serial_fallbacks", C.c_uint64),
+                ("untiled_markers", C.c_uint64), ("dropped_tiles", C.c_uint64)]
 
 
 class AssemblyCounters(C.Structure):

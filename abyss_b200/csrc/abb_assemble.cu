@@ -597,12 +597,12 @@ k_extend(const uint8_t* __restrict__ bases, const uint64_t* __restrict__ offs, c
 // Tiles (abb_walk.cuh): marker enumeration, production, and the repeat check that guards them
 // ------------------------------------------------------------------------------------------
 /** every valid, solid k-mer slot whose canonical hash is a marker and that is not yet in the marker
- *  set joins the list of new markers as (read, window) */
+ *  set joins the list of new markers as (read, window); markers the full set has no room for are counted in n_no_room */
 __global__ void __launch_bounds__(256)
 k_find_markers(const uint64_t* __restrict__ h0, const uint8_t* __restrict__ valid, const uint64_t* __restrict__ slot_offs,
                uint64_t n_reads, uint64_t n_slots, WalkCfg w, const __grid_constant__ HashCfg cfg, unsigned long long* mset,
                unsigned mset_mask, unsigned long long* __restrict__ out /* packed (read << 24 | pos) */, unsigned* n_out,
-               unsigned out_cap, unsigned world, unsigned rank)
+               unsigned out_cap, unsigned* n_no_room, unsigned world, unsigned rank)
 {
 	for (uint64_t s = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; s < n_slots; s += (uint64_t)gridDim.x * blockDim.x) {
 		const uint64_t h = h0[s];
@@ -615,18 +615,10 @@ k_find_markers(const uint64_t* __restrict__ h0, const uint8_t* __restrict__ vali
 			solid &= __ldcg(w.counters + nth_pos(h, cfg, i)) >= w.threshold;
 		if (!solid)
 			continue;
-		const unsigned long long key = h ? h : 1;
-		bool fresh = false;
-		for (uint64_t t = pathset_slot(key, mset_mask + 1);; t = (t + 1) & mset_mask) {
-			const unsigned long long old = atomicCAS(mset + t, 0ULL, key);
-			if (old == 0ULL) {
-				fresh = true;
-				break;
-			}
-			if (old == key)
-				break;
-		}
-		if (!fresh)
+		const unsigned ins = marker_set_insert(mset, mset_mask, h);
+		if (ins == MARKER_NO_ROOM)
+			atomicAdd(n_no_room, 1u); // per window: a marker seen in several windows is counted each time
+		if (ins != MARKER_FRESH)
 			continue;
 		// which read does slot s belong to? upper_bound over slot_offs
 		uint64_t lo = 0, hi = n_reads;
@@ -659,7 +651,7 @@ template <int KW>
 __global__ void __launch_bounds__(kWalkWarps * 32)
 k_make_tiles(const uint8_t* __restrict__ bases, const uint64_t* __restrict__ offs, const unsigned long long* __restrict__ markers,
              unsigned n_markers, unsigned* work, WalkCfg w, const __grid_constant__ HashCfg cfg, Frame* frames, uint64_t* look,
-             uint8_t* stage_bases, uint64_t* stage_hashes, TileStore ts)
+             uint8_t* stage_bases, uint64_t* stage_hashes, TileStore ts, unsigned* n_dropped)
 {
 	const unsigned gwarp = blockIdx.x * kWalkWarps + (threadIdx.x >> 5);
 	WarpCtx c = make_ctx(w, &cfg, frames, look, gwarp, nullptr, 0, nullptr);
@@ -694,8 +686,11 @@ k_make_tiles(const uint8_t* __restrict__ bases, const uint64_t* __restrict__ off
 		}
 		off = __shfl_sync(0xffffffffu, off, 0);
 		idx = __shfl_sync(0xffffffffu, idx, 0);
-		if (off + bytes > ts.pool_size || idx >= ts.cap)
+		if (off + bytes > ts.pool_size || idx >= ts.cap) {
+			if (c.lane == 0)
+				atomicAdd(n_dropped, 1u);
 			continue; // store full: same graceful degradation
+		}
 		uint64_t* dh = reinterpret_cast<uint64_t*>(ts.pool + off);
 		uint8_t* db = ts.pool + off + 8ULL * t.n;
 		for (unsigned i = c.lane; i < t.n; i += 32) {
@@ -1213,7 +1208,7 @@ struct abb_assembler {
 	unsigned tile_cap = 0;
 	DevBuf<unsigned> d_tile_tab;
 	unsigned tile_tab_mask = 0;
-	DevBuf<unsigned> d_tile_n; // [0] tiles stored, [1] work counter, [2] new markers
+	DevBuf<unsigned> d_tile_n; // [0] tiles stored, [1] work counter, [2] new markers, [3] markers without room, [4] tiles dropped
 	DevBuf<uint8_t> d_tile_pool;
 	unsigned long long tile_pool_size = 0;
 	DevBuf<unsigned long long> d_tile_pool_top;
@@ -1246,6 +1241,7 @@ struct abb_assembler {
 namespace {
 
 constexpr unsigned kMaxSpec = 1024;
+constexpr unsigned kTileCounters = 5; // the words of abb_assembler::d_tile_n
 constexpr unsigned kMinSpec = 256;   // with tiles a round costs about the same latency for 64 or 1024 walkers, and wasted walks are cheap
 constexpr unsigned long long kArenaDefault = 4ULL << 30;
 static unsigned long long g_arena_hint = 0; // the arena size the previous assembler of this process ended up needing
@@ -1394,8 +1390,8 @@ int ensure_tile_store(abb_assembler* a)
 	ABB_CHECK(marker_set.alloc(mset));
 	ABB_CUDA(cudaMemsetAsync(marker_set.p, 0, mset * sizeof(unsigned long long), a->stream));
 	ABB_CHECK(tile_pool.alloc(pool));
-	ABB_CHECK(tile_n.alloc(4));
-	ABB_CUDA(cudaMemsetAsync(tile_n.p, 0, 4 * sizeof(unsigned), a->stream));
+	ABB_CHECK(tile_n.alloc(kTileCounters));
+	ABB_CUDA(cudaMemsetAsync(tile_n.p, 0, kTileCounters * sizeof(unsigned), a->stream));
 	ABB_CHECK(pool_top.alloc(1));
 	ABB_CUDA(cudaMemsetAsync(pool_top.p, 0, sizeof(unsigned long long), a->stream));
 	a->d_tiles = std::move(tiles);
@@ -1474,18 +1470,18 @@ int produce_tiles(abb_assembler* a, uint64_t n_reads, uint64_t n_slots)
 	const unsigned world = a->world(), rank = a->rank();
 	const unsigned out_cap = (unsigned)std::min<uint64_t>(n_slots / (kMarkerMask + 1) * 2 + 4096, a->marker_set_mask / 2 + 1);
 	ABB_CHECK(a->new_markers.reserve(out_cap));
-	ABB_CUDA(cudaMemsetAsync(a->d_tile_n.p + 1, 0, 2 * sizeof(unsigned), st));
+	ABB_CUDA(cudaMemsetAsync(a->d_tile_n.p + 1, 0, (kTileCounters - 1) * sizeof(unsigned), st));
 	k_find_markers<<<a->sms * 16, 256, 0, st>>>(a->h0.p, a->valid.p, a->slot_offs.p, n_reads, n_slots, w, f->cfg, a->d_marker_set.p,
-	                                         a->marker_set_mask, a->new_markers.p, a->d_tile_n.p + 2, out_cap, world, rank);
+	                                         a->marker_set_mask, a->new_markers.p, a->d_tile_n.p + 2, out_cap, a->d_tile_n.p + 3,
+	                                         world, rank);
 	ABB_CUDA(cudaGetLastError());
-	unsigned nm = 0, n0 = 0;
+	unsigned tn[kTileCounters] = {};
 	unsigned long long p0 = 0;
-	ABB_CUDA(cudaMemcpyAsync(&nm, a->d_tile_n.p + 2, sizeof nm, cudaMemcpyDeviceToHost, st));
-	ABB_CUDA(cudaMemcpyAsync(&n0, a->d_tile_n.p, sizeof n0, cudaMemcpyDeviceToHost, st));
+	ABB_CUDA(cudaMemcpyAsync(tn, a->d_tile_n.p, sizeof tn, cudaMemcpyDeviceToHost, st));
 	ABB_CUDA(cudaMemcpyAsync(&p0, a->d_tile_pool_top.p, sizeof p0, cudaMemcpyDeviceToHost, st));
 	ABB_CUDA(cudaStreamSynchronize(st));
-	nm = std::min(nm, out_cap);
-	n0 = std::min(n0, a->tile_cap);
+	const unsigned nm = std::min(tn[2], out_cap), n0 = std::min(tn[0], a->tile_cap);
+	a->st.untiled_markers += tn[3] + (tn[2] - nm); // no room in the marker set, or beyond the new-marker list
 	a->st.launches += 1;
 	if (nm == 0 && world == 1)
 		return ABB_OK;
@@ -1500,16 +1496,16 @@ int produce_tiles(abb_assembler* a, uint64_t n_reads, uint64_t n_slots)
 			             a->d_tile_pool_top.p };
 		ABB_DISPATCH_KW(a->kw, (k_make_tiles<KW><<<grid, kWalkWarps * 32, 0, st>>>(a->cur_bases, a->cur_offs, a->new_markers.p, nm,
 		                                                                          a->d_tile_n.p + 1, w, f->cfg, a->frames.p, a->look.p,
-		                                                                          a->stage_bases.p, a->stage_hashes.p, ts)));
+		                                                                          a->stage_bases.p, a->stage_hashes.p, ts, a->d_tile_n.p + 4)));
 		ABB_CUDA(cudaGetLastError());
 		a->st.launches += 1;
 	}
-	unsigned nt = 0;
 	unsigned long long p1 = 0;
-	ABB_CUDA(cudaMemcpyAsync(&nt, a->d_tile_n.p, sizeof nt, cudaMemcpyDeviceToHost, st));
+	ABB_CUDA(cudaMemcpyAsync(tn, a->d_tile_n.p, sizeof tn, cudaMemcpyDeviceToHost, st));
 	ABB_CUDA(cudaMemcpyAsync(&p1, a->d_tile_pool_top.p, sizeof p1, cudaMemcpyDeviceToHost, st));
 	ABB_CUDA(cudaStreamSynchronize(st));
-	nt = std::min(nt, a->tile_cap);
+	unsigned nt = std::min(tn[0], a->tile_cap);
+	a->st.dropped_tiles += tn[4];
 	p1 = std::min(p1, a->tile_pool_size);
 	a->st.markers += nm;
 	a->st.tiles = nt;
@@ -2216,7 +2212,7 @@ int abb_assembler_reset(abb_assembler* a)
 	if (a->d_tile_tab.p) { // the tiles describe the old contents of the solid filter: forget them, keep the memory
 		ABB_CUDA(cudaMemsetAsync(a->d_tile_tab.p, 0, ((size_t)a->tile_tab_mask + 1) * sizeof(unsigned), st));
 		ABB_CUDA(cudaMemsetAsync(a->d_marker_set.p, 0, ((size_t)a->marker_set_mask + 1) * sizeof(unsigned long long), st));
-		ABB_CUDA(cudaMemsetAsync(a->d_tile_n.p, 0, 4 * sizeof(unsigned), st));
+		ABB_CUDA(cudaMemsetAsync(a->d_tile_n.p, 0, kTileCounters * sizeof(unsigned), st));
 		ABB_CUDA(cudaMemsetAsync(a->d_tile_pool_top.p, 0, sizeof(unsigned long long), st));
 	}
 	ABB_CUDA(cudaStreamSynchronize(st));

@@ -737,6 +737,33 @@ enum TileStop : uint8_t { TS_MARKER = 0, TS_CODE = 1, TS_CAP = 2 };
 
 ABB_HD bool is_marker(uint64_t canon) { return (canon & kMarkerMask) == 0; }
 
+/** the set of markers that already have tiles: open addressing over mask + 1 entries of 64-bit keys, 0 = empty */
+constexpr unsigned kMarkerProbes = 64; // probe bound: a full set answers MARKER_NO_ROOM instead of probing forever
+enum MarkerInsert : unsigned { MARKER_SEEN = 0, MARKER_FRESH = 1, MARKER_NO_ROOM = 2 };
+
+/** enter marker `canon` into the set.  Exactly one caller per key gets MARKER_FRESH (and makes its tiles).  A key that
+ *  finds neither itself nor a free entry within kMarkerProbes probes gets MARKER_NO_ROOM and stays without tiles; walks
+ *  pass it vertex by vertex.  Entries are never removed and a key is only ever stored within kMarkerProbes entries of
+ *  its home slot, so the bound cannot hide a stored key: a key is fresh at most once. */
+ABB_HD unsigned marker_set_insert(unsigned long long* set, unsigned mask, uint64_t canon)
+{
+	const unsigned long long key = canon ? canon : 1; // 0 marks an empty entry; 1 is no marker, so no marker collides with it
+	uint64_t t = pathset_slot(key, mask + 1);
+	for (unsigned i = 0; i < kMarkerProbes; ++i, t = (t + 1) & mask) {
+#if defined(__CUDA_ARCH__)
+		const unsigned long long old = atomicCAS(set + t, 0ULL, key);
+#else
+		unsigned long long old = 0;
+		__atomic_compare_exchange_n(set + t, &old, key, false, __ATOMIC_SEQ_CST, __ATOMIC_SEQ_CST);
+#endif
+		if (old == 0ULL)
+			return MARKER_FRESH;
+		if (old == key)
+			return MARKER_SEEN;
+	}
+	return MARKER_NO_ROOM;
+}
+
 struct TileRec {
 	uint64_t key;        // canonical hash of the marker
 	uint64_t lb_t;       // canonical hash of LB's unique predecessor (valid if lb_code == ER_LENGTH_LIMIT)

@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define ABB_VERSION 100
+#define ABB_VERSION 101
 
 enum {
 	ABB_OK = 0,
@@ -282,6 +282,9 @@ typedef struct abb_assembly_stats {
 	float ms_total, ms_cand;    /* host wall clock of the process_reads calls / of building the candidate list */
 	uint64_t markers, tiles;    /* marker vertices found / marker-to-marker tiles stored */
 	uint64_t serial_fallbacks;  /* reads re-walked vertex by vertex after the repeat check */
+	/* the tile store is bounded; what does not fit gets no tiles and is walked vertex by vertex (same output, slower) */
+	uint64_t untiled_markers;   /* marker windows that found no room in the marker set, plus new markers beyond the list */
+	uint64_t dropped_tiles;     /* tiles computed but not stored: the tile records or the tile pool were full */
 } abb_assembly_stats;
 int abb_assembler_stats(const abb_assembler* a, abb_assembly_stats* out);
 

@@ -7,6 +7,10 @@
 // golden FASTA on a machine without a GPU.  The counting filter is built with the C oracle.
 //
 //   host_walk K KC H COUNTERS TRIM reads.fq [readlog.tsv] > out.fa
+//   host_walk markerset                 checks marker_set_insert on sets it fills up
+//
+// HOST_WALK_TILES=1 splices tiles as the kernels do; HOST_WALK_DROP_TILES=SEED then leaves out a seeded subset of the tiles,
+// as a full tile store does on the GPU: one of the four tiles of some markers, all four of others.
 #include "../../abyss_b200/csrc/abb_walk.cuh"
 extern "C" {
 #include "../../oracle/abyss_oracle.h"
@@ -289,6 +293,14 @@ struct Assembly {
 	}
 };
 
+static uint64_t splitmix64(uint64_t x)
+{
+	x += 0x9E3779B97F4A7C15ULL;
+	x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ULL;
+	x = (x ^ (x >> 27)) * 0x94D049BB133111EBULL;
+	return x ^ (x >> 31);
+}
+
 template <int KW>
 static int run(unsigned k, unsigned kc, unsigned H, uint64_t m, unsigned trim, const char* path, const char* logpath)
 {
@@ -342,7 +354,17 @@ static int run(unsigned k, unsigned kc, unsigned H, uint64_t m, unsigned trim, c
 		// markers = solid k-mers of the reads whose canonical hash has its low bits clear; 4 tiles each
 		std::vector<uint8_t> sb(kTileCap);
 		std::vector<uint64_t> sh(kTileCap);
-		std::unordered_set<uint64_t> seen;
+		// the marker set sized as ensure_tile_store would for every window being solid: it never fills here
+		uint64_t windows = 0;
+		for (auto& s : seqs)
+			windows += s.size() >= k ? s.size() - k + 1 : 0;
+		unsigned mset_cap = 1;
+		while (mset_cap < (windows / (kMarkerMask + 1) * 2 + 4096) * 4)
+			mset_cap <<= 1;
+		std::vector<unsigned long long> mset(mset_cap, 0);
+		const char* drop = getenv("HOST_WALK_DROP_TILES");
+		const uint64_t drop_seed = drop ? strtoull(drop, nullptr, 10) : 0;
+		size_t n_markers = 0, dropped = 0, lost_one = 0, lost_all = 0;
 		for (auto& s : seqs) {
 			if (s.size() < k)
 				continue;
@@ -350,10 +372,27 @@ static int run(unsigned k, unsigned kc, unsigned H, uint64_t m, unsigned trim, c
 				if (s.find_first_not_of("ACGT", j) < j + k)
 					continue;
 				Vtx<KW> v = vtx_from_codes<KW>((const uint8_t*)s.data() + j, k, true, c.rt);
-				if (!is_marker(v.canon()) || !c.contains(v.bloom()) || !seen.insert(v.canon()).second)
+				if (!is_marker(v.canon()) || !c.contains(v.bloom()))
 					continue;
+				const unsigned ins = marker_set_insert(mset.data(), mset_cap - 1, v.canon());
+				if (ins == MARKER_NO_ROOM) {
+					fprintf(stderr, "host_walk: marker set full\n");
+					return 4;
+				}
+				if (ins != MARKER_FRESH)
+					continue;
+				++n_markers;
+				// 1 marker in 8 loses one of its tiles, 1 in 8 all four
+				const uint64_t r = drop ? splitmix64(drop_seed ^ v.canon()) : 0;
+				const unsigned drop_mask = !drop ? 0u : (r & 7) == 0 ? 15u : (r & 7) == 1 ? 1u << ((r >> 3) & 3) : 0u;
+				lost_one += drop_mask && drop_mask != 15u;
+				lost_all += drop_mask == 15u;
 				const Vtx<KW> rc = vtx_revcomp(v, k);
 				for (int w = 0; w < 4; ++w) {
+					if (drop_mask >> w & 1) {
+						++dropped;
+						continue;
+					}
 					TileRec t;
 					memset(&t, 0, sizeof t);
 					make_tile(c, (w & 2) ? rc : v, (w & 1) ? REV : FWD, &t, sb.data(), sh.data());
@@ -380,7 +419,8 @@ static int run(unsigned k, unsigned kc, unsigned H, uint64_t m, unsigned trim, c
 				}
 			}
 		c.tile_splices = 0;
-		fprintf(stderr, "host_walk: %zu tiles from %zu markers, %zu linked\n", c.tile_recs.size(), seen.size(), linked);
+		fprintf(stderr, "host_walk: %zu tiles from %zu markers, %zu linked, %zu dropped (%zu markers lost one tile, %zu all four)\n",
+		        c.tile_recs.size(), n_markers, linked, dropped, lost_one, lost_all);
 	}
 
 	Assembly as;
@@ -472,8 +512,50 @@ static int run(unsigned k, unsigned kc, unsigned H, uint64_t m, unsigned trim, c
 	return 0;
 }
 
+/** marker_set_insert on sets it fills: every key is fresh exactly once, a full set answers MARKER_NO_ROOM (the loop is bounded
+ *  by construction, so the check is that the answer is right), and keys stored before the set filled up are still found */
+static int markerset_check()
+{
+	int bad = 0;
+	for (unsigned cap : { 64u, 128u, 4096u }) {
+		std::vector<unsigned long long> set(cap, 0);
+		std::unordered_set<uint64_t> fresh;
+		std::vector<uint64_t> keys;
+		unsigned no_room = 0, seen_twice = 0;
+		for (uint64_t i = 0; i < 4ull * cap; ++i) {
+			const uint64_t key = splitmix64(i) & ~kMarkerMask; // markers; key 0 (stored as 1) comes first
+			keys.push_back(i == 0 ? 0 : key);
+			const unsigned r = marker_set_insert(set.data(), cap - 1, keys.back());
+			if (r == MARKER_FRESH && !fresh.insert(keys.back()).second)
+				++seen_twice;
+			no_room += r == MARKER_NO_ROOM;
+			if (cap <= kMarkerProbes && r == MARKER_NO_ROOM && fresh.size() < cap) {
+				fprintf(stderr, "markerset: cap %u: no room with %zu of %u entries taken\n", cap, fresh.size(), cap);
+				++bad;
+			}
+		}
+		// a second pass: nothing is fresh any more, every key stored before is found
+		unsigned refound = 0;
+		for (uint64_t key : keys) {
+			const unsigned r = marker_set_insert(set.data(), cap - 1, key);
+			if (r == MARKER_FRESH)
+				++seen_twice;
+			refound += r == MARKER_SEEN && fresh.count(key);
+		}
+		const bool full = fresh.size() == cap || (cap > kMarkerProbes && no_room > 0);
+		printf("cap %u fresh %zu no_room %u refound %u twice %u\n", cap, fresh.size(), no_room, refound, seen_twice);
+		if (seen_twice || !full || fresh.size() > cap || refound < fresh.size() || !no_room) {
+			fprintf(stderr, "markerset: cap %u failed\n", cap);
+			++bad;
+		}
+	}
+	return bad ? 1 : 0;
+}
+
 int main(int argc, char** argv)
 {
+	if (argc == 2 && !strcmp(argv[1], "markerset"))
+		return markerset_check();
 	if (argc < 7) {
 		fprintf(stderr, "usage: host_walk K KC H COUNTERS TRIM reads.fq [readlog]\n");
 		return 2;

@@ -21,7 +21,7 @@ def test_header_symbols_exported(abb):
     for n in names:
         assert hasattr(lib, n), f"{n} declared in include/abyss_b200.h but not exported"
         assert n in abb.SIGNATURES, f"{n} has no ctypes signature in abyss_b200/capi.py"
-    assert lib.abb_version() == 100
+    assert lib.abb_version() == 101
 
 
 def test_no_cpu_fallback(abb):
@@ -90,10 +90,30 @@ def test_header_is_plain_c(tmp_path):
     r = subprocess.run([str(exe)], capture_output=True, text=True)
     assert r.returncode == 0, r.stderr
     lines = r.stdout.split("\n")
-    assert lines[0] == "100"
+    assert lines[0] == "101"
     import torch
     if not torch.cuda.is_available():
         assert lines[1].startswith("-2 -2 ") and "no CPU fallback" in lines[1]  # ABB_ENODEV from both entry points
+
+
+def test_assembly_stats_mirror_matches_header(tmp_path, abb):
+    # capi.AssemblyStats mirrors abb_assembly_stats field by field: a field added to one and not the other shifts every later
+    # field, so the size and the offset of every field must agree with what a C compiler makes of the header
+    import ctypes
+    import subprocess
+    fields = [f for f, _ in abb.AssemblyStats._fields_]
+    src = tmp_path / "stats_layout.c"
+    src.write_text('#include "abyss_b200.h"\n#include <stddef.h>\n#include <stdio.h>\nint main(void) {\n'
+                   '    printf("%zu\\n", sizeof(abb_assembly_stats));\n'
+                   + "".join(f'    printf("%zu\\n", offsetof(abb_assembly_stats, {f}));\n' for f in fields)
+                   + "    return 0;\n}\n")
+    exe = tmp_path / "stats_layout"
+    subprocess.run(["gcc", "-std=c99", "-Wall", "-Werror", "-I" + os.path.join(ROOT, "include"), "-o", str(exe), str(src)], check=True,
+                   capture_output=True)
+    got = [int(x) for x in subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.split()]
+    assert got[0] == ctypes.sizeof(abb.AssemblyStats)
+    assert got[1:] == [getattr(abb.AssemblyStats, f).offset for f in fields]
+    assert fields[-2:] == ["untiled_markers", "dropped_tiles"]
 
 
 def test_bench_derived_rooflines():

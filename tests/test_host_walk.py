@@ -6,6 +6,7 @@ traversal logic be verified on a machine without a GPU."""
 import gzip
 import json
 import os
+import re
 import subprocess
 
 import pytest
@@ -65,3 +66,38 @@ def test_spaced_seeds(host_walk, tmp_path, case):
     want = open(os.path.join(GOLD, case["name"] + ".fa")).read()
     assert got.count(">") == case["n_contigs"]
     assert got == want
+
+
+def test_marker_set_full(host_walk):
+    # marker_set_insert (abb_walk.cuh, the insert of k_find_markers) on 64-, 128- and 4096-entry sets filled past capacity:
+    # a full set answers "no room" instead of probing forever, no key is ever fresh twice, and keys stored earlier are found
+    r = subprocess.run([host_walk, "markerset"], capture_output=True, text=True)
+    assert r.returncode == 0, r.stdout + r.stderr
+    assert r.stdout.startswith("cap 64 fresh 64 no_room 192 refound 64 twice 0\n")
+
+
+def _cyc_reads(tmp_path, case):
+    b = case["b"]
+    n = int(b / 1.125 + 0.5)  # counters_for_budget
+    return _reads(tmp_path, case["reads"]), n if n % 64 == 0 else n + 64 - n % 64
+
+
+@pytest.mark.parametrize("name", ["e2e_g10k_k25_small", "cyc_circ_k25"])
+@pytest.mark.parametrize("seed", [1, 7])
+def test_dropped_tiles_same_output(host_walk, tmp_path, name, seed):
+    # what a full tile store leaves behind: markers missing one of their four tiles, markers missing all four.  Walks pass
+    # them vertex by vertex and the unitigs stay the reference's
+    if name.startswith("cyc_"):
+        c = {c["name"]: c for c in json.load(open(os.path.join(GOLD, "cyc_cases.json")))}[name]
+        reads, counters = _cyc_reads(tmp_path, c)
+        trim = c["trim"]
+    else:
+        c = {c["name"]: c for c in json.load(open(os.path.join(GOLD, "e2e_cases.json")))}[name]
+        reads, counters, trim = _reads(tmp_path, name), c["counters"], c["k"]
+    env = dict(os.environ, HOST_WALK_MASK="", HOST_WALK_TILES="1", HOST_WALK_DROP_TILES=str(seed))
+    r = subprocess.run([host_walk, str(c["k"]), str(c["kc"]), str(c["H"]), str(counters), str(trim), reads], capture_output=True,
+                       text=True, env=env)
+    assert r.returncode == 0, r.stderr
+    m = re.search(r"(\d+) dropped \((\d+) markers lost one tile, (\d+) all four\)", r.stderr)
+    assert m and int(m.group(2)) > 0 and int(m.group(3)) > 0, r.stderr
+    assert r.stdout == open(os.path.join(GOLD, name + ".fa")).read()

@@ -368,8 +368,11 @@ static int run(unsigned k, unsigned kc, unsigned H, uint64_t m, unsigned trim, c
 		for (auto& s : seqs) {
 			if (s.size() < k)
 				continue;
+			size_t bad = s.find_first_not_of("ACGT"); // the first non-ACGT base at or after j: one scan per read, not per window
 			for (size_t j = 0; j + k <= s.size(); ++j) {
-				if (s.find_first_not_of("ACGT", j) < j + k)
+				if (bad < j)
+					bad = s.find_first_not_of("ACGT", j);
+				if (bad < j + k)
 					continue;
 				Vtx<KW> v = vtx_from_codes<KW>((const uint8_t*)s.data() + j, k, true, c.rt);
 				if (!is_marker(v.canon()) || !c.contains(v.bloom()))

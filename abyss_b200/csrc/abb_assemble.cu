@@ -391,7 +391,7 @@ struct ContigRec {
 	unsigned seed_pos;
 	unsigned psize;
 	unsigned char left, right, flags, pad1; // flags: 1 pushed_front, 2 pushed_back, 4 popped_front, 8 popped_back
-	unsigned long long front_h, back_h;     // canonical hashes of trimmed-off end vertices (flags 4 / 8)
+	unsigned long long front_h, back_h;     // Bloom hashes of trimmed-off end vertices (flags 4 / 8), as ch0 holds them
 	unsigned left_n, right_n;               // vertices added by the two extensions (-T trace)
 };
 
@@ -416,8 +416,8 @@ struct DevEmit {
 				r.right = (unsigned char)o.right;
 				r.flags = (unsigned char)((o.pushed_front ? 1 : 0) | (o.pushed_back ? 2 : 0) | (o.popped_front ? 4 : 0) | (o.popped_back ? 8 : 0));
 				r.pad1 = 0;
-				r.front_h = o.front_h;
-				r.back_h = o.back_h;
+				r.front_h = o.front_b;
+				r.back_h = o.back_b;
 				r.left_n = o.left_n;
 				r.right_n = o.right_n;
 				recs[idx] = r;
@@ -596,23 +596,27 @@ k_extend(const uint8_t* __restrict__ bases, const uint64_t* __restrict__ offs, c
 // ------------------------------------------------------------------------------------------
 // Tiles (abb_walk.cuh): marker enumeration, production, and the repeat check that guards them
 // ------------------------------------------------------------------------------------------
-/** every valid, solid k-mer slot whose canonical hash is a marker and that is not yet in the marker
- *  set joins the list of new markers as (read, window); markers the full set has no room for are counted in n_no_room */
+/** every valid, solid k-mer slot whose tile_key is a marker and that is not yet in the marker set joins the list of new
+ *  markers as (read, window); markers the full set has no room for are counted in n_no_room.  key/valid: the unmasked
+ *  canonical hash and full-ACGT flag of each window (tile_key); bloom: the hash the solid filter is probed with.  Without
+ *  a spaced seed key and bloom are the same array. */
 __global__ void __launch_bounds__(256)
-k_find_markers(const uint64_t* __restrict__ h0, const uint8_t* __restrict__ valid, const uint64_t* __restrict__ slot_offs,
-               uint64_t n_reads, uint64_t n_slots, WalkCfg w, const __grid_constant__ HashCfg cfg, unsigned long long* mset,
-               unsigned mset_mask, unsigned long long* __restrict__ out /* packed (read << 24 | pos) */, unsigned* n_out,
-               unsigned out_cap, unsigned* n_no_room, unsigned world, unsigned rank)
+k_find_markers(const uint64_t* __restrict__ key, const uint8_t* __restrict__ valid, const uint64_t* __restrict__ bloom,
+               const uint64_t* __restrict__ slot_offs, uint64_t n_reads, uint64_t n_slots, WalkCfg w,
+               const __grid_constant__ HashCfg cfg, unsigned long long* mset, unsigned mset_mask,
+               unsigned long long* __restrict__ out /* packed (read << 24 | pos) */, unsigned* n_out, unsigned out_cap,
+               unsigned* n_no_room, unsigned world, unsigned rank)
 {
 	for (uint64_t s = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; s < n_slots; s += (uint64_t)gridDim.x * blockDim.x) {
-		const uint64_t h = h0[s];
+		const uint64_t h = key[s];
 		if (!is_marker(h) || !valid[s])
 			continue;
 		if (world > 1 && (unsigned)((h >> 8) % world) != rank) // several GPUs: each marker is tiled by exactly one rank
 			continue;
+		const uint64_t hb = bloom[s];
 		bool solid = true;
 		for (unsigned i = 0; i < cfg.H; ++i)
-			solid &= __ldcg(w.counters + nth_pos(h, cfg, i)) >= w.threshold;
+			solid &= __ldcg(w.counters + nth_pos(hb, cfg, i)) >= w.threshold;
 		if (!solid)
 			continue;
 		const unsigned ins = marker_set_insert(mset, mset_mask, h);
@@ -779,7 +783,9 @@ k_link_tiles(TileRec* recs, unsigned n, const unsigned* __restrict__ tab, unsign
 /** a canonical hash occurring twice in one (untrimmed) path means the tile splice skipped an
  *  ER_CYCLE: flag the contig.  Every contig has its own open-addressing region
  *  [tab_off[c], tab_off[c+1]) keyed by the full 64-bit canonical hash, so a hit is a genuine repeat
- *  (a false alarm would cost a vertex-by-vertex walk of a possibly Mbp-long unitig). */
+ *  (a false alarm would cost a vertex-by-vertex walk of a possibly Mbp-long unitig).  The hash is the
+ *  Bloom hash ch0; with a spaced seed two vertices with equal identity canon() have equal Bloom hashes,
+ *  so every repeat the reference reports as ER_CYCLE is still found. */
 __global__ void __launch_bounds__(256)
 k_repeat_check(const ContigRec* __restrict__ recs, unsigned n_contigs, const uint64_t* __restrict__ cslot,
                const uint64_t* __restrict__ ch0, unsigned long long* tab, const uint64_t* __restrict__ tab_off,
@@ -1215,6 +1221,8 @@ struct abb_assembler {
 	DevBuf<unsigned long long> d_marker_set;
 	unsigned marker_set_mask = 0;
 	DevBuf<unsigned long long> new_markers, rep_tab;
+	DevBuf<uint64_t> key_h0;  // spaced seed only: unmasked canonical hash (tile_key) of every window of the batch
+	DevBuf<uint8_t> key_valid; // and whether all k bases of the window are ACGT
 	DevBuf<TileRec> tile_export;
 	DevBuf<uint8_t> stage_bases, rep_flag;
 	DevBuf<uint64_t> stage_hashes;
@@ -1471,7 +1479,19 @@ int produce_tiles(abb_assembler* a, uint64_t n_reads, uint64_t n_slots)
 	const unsigned out_cap = (unsigned)std::min<uint64_t>(n_slots / (kMarkerMask + 1) * 2 + 4096, a->marker_set_mask / 2 + 1);
 	ABB_CHECK(a->new_markers.reserve(out_cap));
 	ABB_CUDA(cudaMemsetAsync(a->d_tile_n.p + 1, 0, (kTileCounters - 1) * sizeof(unsigned), st));
-	k_find_markers<<<a->sms * 16, 256, 0, st>>>(a->h0.p, a->valid.p, a->slot_offs.p, n_reads, n_slots, w, f->cfg, a->d_marker_set.p,
+	const uint64_t* key = a->h0.p;
+	const uint8_t* key_valid = a->valid.p;
+	if (a->rt.nmask) {
+		// spaced seed: h0 is the masked Bloom hash and valid covers only the '1' positions, but markers are named by the full
+		// k-mer.  One more streaming pass of the unmasked K1 over the batch gives each window its tile_key and full validity.
+		ABB_CHECK(a->key_h0.reserve(n_slots + 1));
+		ABB_CHECK(a->key_valid.reserve(n_slots + 1));
+		ABB_CHECK(launch_hash(f->k, nullptr, a->cur_bases, a->cur_offs, a->slot_offs.p, 0, n_reads, 0, a->key_h0.p, a->key_valid.p, st,
+		                      &a->st.launches));
+		key = a->key_h0.p;
+		key_valid = a->key_valid.p;
+	}
+	k_find_markers<<<a->sms * 16, 256, 0, st>>>(key, key_valid, a->h0.p, a->slot_offs.p, n_reads, n_slots, w, f->cfg, a->d_marker_set.p,
 	                                         a->marker_set_mask, a->new_markers.p, a->d_tile_n.p + 2, out_cap, a->d_tile_n.p + 3,
 	                                         world, rank);
 	ABB_CUDA(cudaGetLastError());
@@ -2031,9 +2051,8 @@ int abb_assembler_create(abb_assembler** out, abb_filter* solid, const abb_assem
 			a->rt.mpos = a->d_mpos.p;
 		}
 	}
-	// tiles are keyed by vertex hash and assume that equal hashes continue identically; with a spaced seed two k-mers
-	// can share the hash and differ on the don't-care positions, so those runs walk vertex by vertex
-	a->tiles_on = getenv("ABB_NO_TILES") == nullptr && solid->mask.empty(); // env: debugging switch
+	// tiles are keyed by the full k-mer (tile_key, abb_walk.cuh), so they serve spaced seeds too
+	a->tiles_on = getenv("ABB_NO_TILES") == nullptr; // env: debugging switch
 	// BloomFilter assembledKmerSet(solid.size(), solid.getHashNum(), solid.getKmerSize()) (bloom-dbg.h:910-911)
 	abb_filter* assembled = nullptr;
 	ABB_CHECK(abb_filter_create(&assembled, ABB_BIT, solid->size, solid->H, solid->k, 0, "", solid->device));

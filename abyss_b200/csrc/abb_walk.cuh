@@ -19,7 +19,9 @@
 // (RollingBloomDBG.h:92-100, RC-invariant).  Here identity is the 64-bit canonical ntHash alone;
 // two distinct k-mers colliding inside one local traversal has probability ~2^-64 per comparison.
 // With a spaced seed (MaskedKmer) a vertex carries the masked Bloom hash and a separate identity (see "Spaced seeds" in
-// DESIGN.md section 3); tiles are switched off then (equal hash no longer implies equal continuation).
+// DESIGN.md section 3).  Two k-mers with the same identity can then differ at a don't-care position and continue
+// differently, so tiles are named by the full k-mer instead (tile_key), while everything the walk compares by vertex
+// identity stays on the identity.
 #pragma once
 #include "abb_device.cuh"
 
@@ -730,12 +732,26 @@ ABB_HD bool bytevec_push(Ctx& c, ByteVec& v, uint8_t x)
 // vertex by vertex would have produced.  The visited set is not consulted while splicing; instead
 // every finished path is checked for a repeated vertex afterwards and, if one is found (cycles,
 // hairpins: rare), that read is walked again without tiles.
+//
+// Markers and tiles are named by tile_key(): the canonical hash of the FULL k-mer.  A walk from a
+// vertex is a function of its full k-mer, the strand held, the direction and the read-only solid
+// filter, so that name is exact (up to the ~2^-64 hash collision).  Without a spaced seed it is the
+// vertex identity canon(); with one, canon() ignores the don't-care positions, and two k-mers that
+// agree on every '1' position but continue differently would share a tile.  The look-behind
+// hashes, the per-vertex hashes a tile stores and the path set stay canon().
 // ------------------------------------------------------------------------------------------
 constexpr uint64_t kMarkerMask = 255;   // 1 vertex in 256 is a marker
 constexpr unsigned kTileCap = 4096;     // longest tile, in pushed vertices
 enum TileStop : uint8_t { TS_MARKER = 0, TS_CODE = 1, TS_CAP = 2 };
 
-ABB_HD bool is_marker(uint64_t canon) { return (canon & kMarkerMask) == 0; }
+ABB_HD bool is_marker(uint64_t key) { return (key & kMarkerMask) == 0; }
+
+/** what tiles and markers are named by: the canonical ntHash of the full k-mer (see above) */
+template <int KW>
+ABB_HD uint64_t tile_key(const Vtx<KW>& v, const RollTab& rt)
+{
+	return rt.nmask == 0 ? v.id : v.h.canonical();
+}
 
 /** the set of markers that already have tiles: open addressing over mask + 1 entries of 64-bit keys, 0 = empty */
 constexpr unsigned kMarkerProbes = 64; // probe bound: a full set answers MARKER_NO_ROOM instead of probing forever
@@ -764,23 +780,26 @@ ABB_HD unsigned marker_set_insert(unsigned long long* set, unsigned mask, uint64
 	return MARKER_NO_ROOM;
 }
 
+/** key, end_key, cls and end_orient name vertices as tiles do (tile_key: the full k-mer); lb_t, prev_last and hashes are
+ *  vertex identities (canon()), compared with what the walk holds.  Without a spaced seed the two are the same value. */
 struct TileRec {
-	uint64_t key;        // canonical hash of the marker
-	uint64_t lb_t;       // canonical hash of LB's unique predecessor (valid if lb_code == ER_LENGTH_LIMIT)
-	uint64_t prev_last;  // canonical hash of the vertex before the last pushed one (the marker itself if n == 1)
-	uint64_t end_key;    // canonical hash of the last pushed vertex
+	uint64_t key;        // tile_key of the marker
+	uint64_t lb_t;       // canon() of LB's unique predecessor (valid if lb_code == ER_LENGTH_LIMIT)
+	uint64_t prev_last;  // canon() of the vertex before the last pushed one (the marker itself if n == 1)
+	uint64_t end_key;    // tile_key of the last pushed vertex
 	uint8_t* bases;      // n pushed bases, in push order
-	uint64_t* hashes;    // n canonical hashes of the pushed vertices
+	uint64_t* hashes;    // n canon() of the pushed vertices
 	uint32_t n;
 	uint32_t next;       // index + 1 of the tile that starts at this tile's end marker (same direction), 0 = look it up
-	uint8_t cls;         // (held orientation is the canonical-hash one) << 1 | direction
+	uint8_t cls;         // vtx_class of the marker as held: (strand of the full canonical k-mer) << 1 | direction
 	uint8_t lb_code;     // ExtCode of LB(marker)
 	uint8_t stop_kind;   // TileStop
 	uint8_t stop_code;   // ExtCode when stop_kind == TS_CODE
-	uint8_t end_orient;  // orientation bit of the last pushed vertex
+	uint8_t end_orient;  // vtx_orient of the last pushed vertex
 	uint8_t pad[3];
 };
 
+/** 1 if the held strand is the one whose unmasked forward hash is tile_key, i.e. the strand of the full canonical k-mer */
 template <int KW>
 ABB_HD unsigned vtx_orient(const Vtx<KW>& v) { return v.h.fh <= v.h.rh ? 1u : 0u; }
 template <int KW>
@@ -864,7 +883,7 @@ ABB_HD void make_tile(Ctx& c, const Vtx<KW>& m, Dir dir, TileRec* t, uint8_t* ba
 			t->lb_t = neighbor_canon(head, c.k, c.rt, opposite(dir), b);
 		}
 	}
-	t->key = m.canon();
+	t->key = tile_key(m, c.rt);
 	t->next = 0;
 	t->cls = (uint8_t)vtx_class(m, dir);
 	unsigned n = 0;
@@ -898,7 +917,7 @@ ABB_HD void make_tile(Ctx& c, const Vtx<KW>& m, Dir dir, TileRec* t, uint8_t* ba
 		c.wr64(hashes + n, head.canon());
 		++n;
 		look_behind = true;
-		if (is_marker(head.canon())) {
+		if (is_marker(tile_key(head, c.rt))) {
 			t->stop_kind = TS_MARKER;
 			break;
 		}
@@ -910,7 +929,7 @@ ABB_HD void make_tile(Ctx& c, const Vtx<KW>& m, Dir dir, TileRec* t, uint8_t* ba
 	}
 	t->n = n;
 	t->prev_last = prev_h;
-	t->end_key = head.canon();
+	t->end_key = tile_key(head, c.rt);
 	t->end_orient = (uint8_t)vtx_orient(head);
 }
 
@@ -967,9 +986,9 @@ ABB_HD ExtCode extend_dir(Ctx& c, Vtx<KW>& head, Dir dir, unsigned* psize, ByteV
 		look_behind = true; // params.lookBehind
 		if (c.failed())
 			return ER_DEAD_END;
-		if (c.tiles_enabled() && is_marker(head.canon())) {
+		if (c.tiles_enabled() && is_marker(tile_key(head, c.rt))) {
 			// splice marker-to-marker tiles for as long as they chain (see the Tiles comment above)
-			uint64_t hk = head.canon();
+			uint64_t hk = tile_key(head, c.rt);
 			unsigned cls = vtx_class(head, dir);
 			bool moved = false;
 			const TileRec* T = c.tile_lookup(hk, cls);
@@ -1052,6 +1071,7 @@ struct ContigOut {
 	bool tip;        // isTip: not output, but its k-mers still count as assembled for this read
 	bool popped_front, popped_back; // a real path vertex (not a pushed duplicate) was trimmed off that end
 	uint64_t front_h, back_h;       // canonical hashes of the trimmed-off vertices
+	uint64_t front_b, back_b;       // their Bloom hashes (the repeat check hashes the contig the way the Bloom filters do)
 	bool pushed_front, pushed_back; // preprocessCircularContig's duplicate vertex survives at that end of seq
 	U32Vec tiles_left, tiles_right; // tiles spliced into the path (their vertices are not in the PathSet)
 };
@@ -1084,6 +1104,7 @@ ABB_HD bool extend_seed(Ctx& c, const Vtx<KW>& seed, PathSet& ps, ContigOut* o)
 	o->tip = is_tip(psize, o->left, o->right, c.trim);
 	o->popped_front = o->popped_back = false;
 	o->front_h = o->back_h = 0;
+	o->front_b = o->back_b = 0;
 
 	// materialise pathToSeq(contigPath): reversed(left) + seed + right, with one spare byte each side
 	// for the vertex preprocessCircularContig may push
@@ -1173,6 +1194,7 @@ ABB_HD bool extend_seed(Ctx& c, const Vtx<KW>& seed, PathSet& ps, ContigOut* o)
 		if (!pushed_front) {
 			o->popped_front = true;
 			o->front_h = front.canon();
+			o->front_b = front.bloom();
 		}
 	} else
 		o->pushed_front = pushed_front;
@@ -1181,6 +1203,7 @@ ABB_HD bool extend_seed(Ctx& c, const Vtx<KW>& seed, PathSet& ps, ContigOut* o)
 		if (!pushed_back) {
 			o->popped_back = true;
 			o->back_h = back.canon();
+			o->back_b = back.bloom();
 		}
 	} else
 		o->pushed_back = pushed_back;

@@ -87,6 +87,8 @@ SIGNATURES = {
     "abb_version": (C.c_int, []),
     "abb_last_error": (C.c_char_p, []),
     "abb_device_count": (C.c_int, []),
+    "abb_set_max_kmer": (C.c_int, [C.c_uint]),
+    "abb_max_kmer": (C.c_uint, []),
     "abb_filter_create": (C.c_int, [C.POINTER(_vp), C.c_int, C.c_uint64, C.c_uint, C.c_uint, C.c_uint, C.c_char_p, C.c_int]),
     "abb_filter_destroy": (C.c_int, [_vp]),
     "abb_konnector_create": (C.c_int, [C.POINTER(_vp), C.c_uint64, C.c_uint, C.c_uint, C.c_uint64, C.c_uint64, C.c_uint64, C.c_int]),
@@ -194,6 +196,15 @@ def fixed_length_reads(ascii_2d: np.ndarray) -> tuple[np.ndarray, np.ndarray]:
 
 def _ptr(a: np.ndarray):
     return a.ctypes.data_as(_vp)
+
+
+def set_max_kmer(max_k: int) -> None:
+    """MAX_KMER of this process (abb_set_max_kmer): k up to max_k (at most 256) is accepted; 192 until it is raised"""
+    check(load().abb_set_max_kmer(max_k))
+
+
+def max_kmer() -> int:
+    return load().abb_max_kmer()
 
 
 def hash_reads(k: int, seqs_or_arrays, mask: str = "", device: int = 0):

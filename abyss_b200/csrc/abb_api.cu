@@ -8,6 +8,7 @@
 #include <nccl.h>
 #include <cub/device/device_scan.cuh>
 #include <algorithm>
+#include <atomic>
 #include <cstdlib>
 #include <cstring>
 #include <new>
@@ -365,6 +366,29 @@ k_count_valid(const uint8_t* __restrict__ valid, uint64_t n, unsigned long long*
 		atomicAdd(out, c);
 }
 
+/** the unmasked K1 over reads with the ring that holds k (see kRingWide) */
+template <int RING>
+static int launch_hash_tma(unsigned k, const uint8_t* d_bases, const uint64_t* d_offs, const uint64_t* d_slot_offs, uint64_t n,
+                           uint64_t slot_base, uint64_t* d_h0, uint8_t* d_valid, cudaStream_t stream)
+{
+	// The opt-in to 16 KB of dynamic shared memory (56 KB in all) is a per-device attribute of the kernel: a process that
+	// drives several GPUs (abyss-bloom-dbg --devices) sets it on each of them.
+	static bool smem_opt_in[64] = {};
+	int dev = 0;
+	ABB_CUDA(cudaGetDevice(&dev));
+	if (!smem_opt_in[dev & 63]) {
+		ABB_CUDA(cudaFuncSetAttribute(k_hash_reads_tma<RING>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * kTmaStage));
+		smem_opt_in[dev & 63] = true;
+	}
+	// read blocks staged into shared memory by the bulk-copy engine (cp.async.bulk), double buffered; the copy needs a
+	// 16-byte aligned source, so reads at an unaligned base pointer are all hashed from global memory
+	const bool may_stage = (reinterpret_cast<uintptr_t>(d_bases) & 15) == 0;
+	const unsigned grid = (unsigned)std::min<uint64_t>((n + kTmaReads - 1) / kTmaReads, (uint64_t)sm_count() * 4);
+	k_hash_reads_tma<RING><<<grid, ring_warps<RING>() * 32, 2 * kTmaStage, stream>>>(d_bases, d_offs, d_slot_offs, slot_base, n, k,
+	                                                                               d_h0, d_valid, may_stage);
+	return ABB_OK;
+}
+
 /** K1 launcher for reads [r0, r1): h0/valid index = slot_offs[r] + j - slot_base */
 int launch_hash(unsigned k, const uint8_t* d_care, const uint8_t* d_bases, const uint64_t* d_offs, const uint64_t* d_slot_offs,
                 uint64_t r0, uint64_t r1, uint64_t slot_base, uint64_t* d_h0, uint8_t* d_valid, cudaStream_t stream, uint64_t* launches)
@@ -377,22 +401,10 @@ int launch_hash(unsigned k, const uint8_t* d_care, const uint8_t* d_bases, const
 		const unsigned grid = (unsigned)std::min<uint64_t>((n + kHashWarps - 1) / kHashWarps, sms * 32);
 		k_hash_reads_masked<<<grid, kHashWarps * 32, 0, stream>>>(d_bases, d_offs + r0, d_slot_offs + r0, slot_base, n, k, d_care,
 		                                                          d_h0, d_valid);
+	} else if (k <= kRingMaxK) {
+		ABB_CHECK(launch_hash_tma<kRing>(k, d_bases, d_offs + r0, d_slot_offs + r0, n, slot_base, d_h0, d_valid, stream));
 	} else {
-		// The opt-in to 16 KB of dynamic shared memory (56 KB in all) is a per-device attribute of the kernel: a process that
-		// drives several GPUs (abyss-bloom-dbg --devices) sets it on each of them.
-		static bool smem_opt_in[64] = {};
-		int dev = 0;
-		ABB_CUDA(cudaGetDevice(&dev));
-		if (!smem_opt_in[dev & 63]) {
-			ABB_CUDA(cudaFuncSetAttribute(k_hash_reads_tma, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * kTmaStage));
-			smem_opt_in[dev & 63] = true;
-		}
-		// read blocks staged into shared memory by the bulk-copy engine (cp.async.bulk), double buffered; the copy needs a
-		// 16-byte aligned source, so reads at an unaligned base pointer are all hashed from global memory
-		const bool may_stage = (reinterpret_cast<uintptr_t>(d_bases) & 15) == 0;
-		const unsigned grid = (unsigned)std::min<uint64_t>((n + kTmaReads - 1) / kTmaReads, sms * 4);
-		k_hash_reads_tma<<<grid, kHashWarps * 32, 2 * kTmaStage, stream>>>(d_bases, d_offs + r0, d_slot_offs + r0, slot_base, n, k,
-		                                                                  d_h0, d_valid, may_stage);
+		ABB_CHECK(launch_hash_tma<kRingWide>(k, d_bases, d_offs + r0, d_slot_offs + r0, n, slot_base, d_h0, d_valid, stream));
 	}
 	if (launches)
 		*launches += 1;
@@ -411,8 +423,11 @@ int launch_hash_segments(unsigned k, const uint8_t* d_care, const uint8_t* d_bas
 	if (d_care)
 		k_hash_segments_masked<<<grid, kHashWarps * 32, 0, stream>>>(d_bases, d_seg_beg, d_seg_len, d_seg_slot, n_segs, k, d_care,
 		                                                             d_h0, d_valid);
-	else
-		k_hash_segments<<<grid, kHashWarps * 32, 0, stream>>>(d_bases, d_seg_beg, d_seg_len, d_seg_slot, n_segs, k, d_h0, d_valid);
+	else if (k <= kRingMaxK)
+		k_hash_segments<kRing><<<grid, kHashWarps * 32, 0, stream>>>(d_bases, d_seg_beg, d_seg_len, d_seg_slot, n_segs, k, d_h0, d_valid);
+	else // half the warps per CTA: twice the CTAs for the same segments per launch
+		k_hash_segments<kRingWide><<<2 * grid, ring_warps<kRingWide>() * 32, 0, stream>>>(d_bases, d_seg_beg, d_seg_len, d_seg_slot,
+		                                                                                   n_segs, k, d_h0, d_valid);
 	ABB_CUDA(cudaGetLastError());
 	return ABB_OK;
 }
@@ -778,6 +793,19 @@ extern "C" {
 int abb_version(void) { return ABB_VERSION; }
 const char* abb_last_error(void) { return g_err; }
 
+/* MAX_KMER of this process: k above it is refused by every entry point that takes a k, as the reference built with
+ * configure --enable-maxk=<max_kmer> refuses it (Common/Kmer.h:44-56) */
+static std::atomic<unsigned> g_max_kmer{ kDefaultMaxK };
+
+int abb_set_max_kmer(unsigned max_k)
+{
+	ABB_REQUIRE(max_k >= 1 && max_k <= kMaxK, "the largest k-mer size must be in 1..%u", kMaxK);
+	g_max_kmer.store(max_k);
+	return ABB_OK;
+}
+
+unsigned abb_max_kmer(void) { return g_max_kmer.load(); }
+
 int abb_device_count(void)
 {
 	int n = 0;
@@ -799,7 +827,7 @@ int abb_filter_create(abb_filter** out, int kind, uint64_t size, unsigned num_ha
 	ABB_REQUIRE(kind != ABB_KONNECTOR, "Konnector filters are created with abb_konnector_create");
 	ABB_REQUIRE(kind == ABB_COUNTING || kind == ABB_BIT || kind == ABB_CASCADING, "unknown filter kind %d", kind);
 	ABB_REQUIRE(num_hashes >= 1 && num_hashes <= kMaxHashes, "number of hash functions must be in 1..%u (MAX_HASHES)", kMaxHashes);
-	ABB_REQUIRE(k >= 1 && k <= kMaxK, "k-mer size must be in 1..%u (MAX_KMER)", kMaxK);
+	ABB_REQUIRE(k >= 1 && k <= abb_max_kmer(), "k-mer size must be in 1..%u (MAX_KMER)", abb_max_kmer());
 	if (kind == ABB_COUNTING) {
 		// CountingBloomFilter ctor pads the byte size to a multiple of 8 (CountingBloomFilter.hpp:40-49)
 		if (size % 8)
@@ -880,7 +908,7 @@ int abb_konnector_create(abb_filter** out, uint64_t full_bits, unsigned k, unsig
 {
 	ABB_REQUIRE(out != nullptr, "abb_konnector_create: out is NULL");
 	*out = nullptr;
-	ABB_REQUIRE(k >= 1 && k <= kMaxK, "k-mer size must be in 1..%u (MAX_KMER)", kMaxK);
+	ABB_REQUIRE(k >= 1 && k <= abb_max_kmer(), "k-mer size must be in 1..%u (MAX_KMER)", abb_max_kmer());
 	ABB_REQUIRE(full_bits >= 2, "a Konnector filter needs at least 2 bits");
 	ABB_REQUIRE(start_bit <= end_bit && end_bit < full_bits, "window [%llu, %llu] is not inside a filter of %llu bits",
 	            (unsigned long long)start_bit, (unsigned long long)end_bit, (unsigned long long)full_bits);
@@ -1417,7 +1445,7 @@ int abb_graph_neighbors(abb_filter* g, const char* kmers, uint64_t n, abb_filter
 int abb_hash_reads(unsigned k, const char* mask, const char* bases, const uint64_t* offsets, uint64_t n_reads,
                    uint64_t* out_h0, uint8_t* out_valid, uint64_t* n_slots_out, int device)
 {
-	ABB_REQUIRE(k >= 1 && k <= kMaxK, "k-mer size must be in 1..%u", kMaxK);
+	ABB_REQUIRE(k >= 1 && k <= abb_max_kmer(), "k-mer size must be in 1..%u", abb_max_kmer());
 	if (n_slots_out)
 		*n_slots_out = 0;
 	if (n_reads == 0)

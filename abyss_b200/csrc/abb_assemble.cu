@@ -1315,7 +1315,8 @@ WalkCfg walk_cfg(const abb_assembler* a)
 		case 2: { constexpr int KW = 2; __VA_ARGS__; } break; \
 		case 3: { constexpr int KW = 3; __VA_ARGS__; } break; \
 		case 4: { constexpr int KW = 4; __VA_ARGS__; } break; \
-		default: { constexpr int KW = 6; __VA_ARGS__; } break; \
+		case 5: case 6: { constexpr int KW = 6; __VA_ARGS__; } break; \
+		default: { constexpr int KW = 8; __VA_ARGS__; } break; \
 		}                                     \
 	} while (0)
 

@@ -29,7 +29,8 @@ constexpr uint64_t kSeedT = 0x295549f54be24456ULL; // :28
 constexpr uint64_t kMultiSeed = 0x90b45d39fb6da1faULL; // :22
 constexpr unsigned kMultiShift = 27;                   // :19
 constexpr unsigned kMaxHashes = 32;                    // configure.ac:151-159 MAX_HASHES
-constexpr unsigned kMaxK = 192;                        // configure.ac MAX_KMER
+constexpr unsigned kMaxK = 256;                        // the largest k the kernels are built for (configure --enable-maxk=256)
+constexpr unsigned kDefaultMaxK = 192;                 // configure.ac MAX_KMER default: the k accepted until abb_set_max_kmer
 
 constexpr uint64_t kMask33 = 0x1FFFFFFFFULL;
 constexpr uint64_t kMask31 = 0x7FFFFFFFULL;

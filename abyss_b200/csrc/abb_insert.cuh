@@ -160,6 +160,13 @@ ABB_D void apply_cascading(const FilterView& f, const uint64_t* pos, unsigned H)
 // ------------------------------------------------------------------------------------------
 constexpr int kHashWarps = 8;     // warps per CTA
 constexpr int kRing = 256;        // per-warp ring of prefix values; needs k + 32 <= 256
+// k = 225..256 needs the next power of two, a 512-entry ring.  Its instances of the ring kernels run half as many warps per
+// CTA, so the rings keep to the same 40 KB of static shared memory (8 x 256 = 4 x 512 entries): no opt-in past 48 KB, and
+// the same number of rings per SM as doubling them behind the opt-in would give.
+constexpr int kRingWide = 512;
+constexpr unsigned kRingMaxK = kRing - 32; // the largest k of the 256-entry ring
+template <int RING>
+constexpr int ring_warps() { return kHashWarps * kRing / RING; }
 
 ABB_D uint64_t shfl_up64(uint64_t v, int d)
 {
@@ -181,7 +188,8 @@ ABB_D uint64_t shfl64(uint64_t v, int src)
  * P_i = XOR_{t<=i} R^{-t}(seed(c_t)), Q_i = XOR_{t<=i} R^{t}(seed(comp c_t)):
  *   fwd(j) = R^{j+k-1}(P_{j+k-1} ^ P_{j-1}),  rc(j) = R^{-j}(Q_{j+k-1} ^ Q_{j-1}).
  */
-/** one warp hashes the L bases at `beg`; window j goes to slot slot0 + j */
+/** one warp hashes the L bases at `beg`; window j goes to slot slot0 + j; needs k + 32 <= RING */
+template <int RING>
 ABB_D void hash_one_read(const uint8_t* __restrict__ bases, uint64_t beg, unsigned L, uint64_t slot0, unsigned k, uint64_t* P,
                          uint64_t* Q, unsigned* B, int lane, uint64_t* __restrict__ h0_out, uint8_t* __restrict__ valid_out)
 {
@@ -210,9 +218,9 @@ ABB_D void hash_one_read(const uint8_t* __restrict__ bases, uint64_t beg, unsign
 		q ^= carryQ;
 		const unsigned badmask = __ballot_sync(0xffffffffu, code >= 4 && i < L);
 		const unsigned b = carryB + __popc(badmask & (0xffffffffu >> (31 - lane)));
-		P[i & (kRing - 1)] = p;
-		Q[i & (kRing - 1)] = q;
-		B[i & (kRing - 1)] = b;
+		P[i & (RING - 1)] = p;
+		Q[i & (RING - 1)] = q;
+		B[i & (RING - 1)] = b;
 		carryP = shfl64(p, 31);
 		carryQ = shfl64(q, 31);
 		carryB += __popc(badmask);
@@ -222,9 +230,9 @@ ABB_D void hash_one_read(const uint8_t* __restrict__ bases, uint64_t beg, unsign
 			uint64_t pj = 0, qj = 0;
 			unsigned bj = 0;
 			if (j > 0) {
-				pj = P[(j - 1) & (kRing - 1)];
-				qj = Q[(j - 1) & (kRing - 1)];
-				bj = B[(j - 1) & (kRing - 1)];
+				pj = P[(j - 1) & (RING - 1)];
+				qj = Q[(j - 1) & (RING - 1)];
+				bj = B[(j - 1) & (RING - 1)];
 			}
 			const uint64_t fh = srol_n(p ^ pj, i);
 			const uint64_t rh = sror_n(q ^ qj, j);
@@ -271,14 +279,16 @@ ABB_D void hash_one_read_masked(const uint8_t* __restrict__ bases, uint64_t beg,
 constexpr unsigned kTmaStage = 8192; // bytes per stage
 constexpr unsigned kTmaReads = 32;   // reads per stage: 32 x 150 bases = 4 800 bytes
 
-static __global__ void __launch_bounds__(kHashWarps * 32)
+template <int RING>
+static __global__ void __launch_bounds__(ring_warps<RING>() * 32)
 k_hash_reads_tma(const uint8_t* __restrict__ bases, const uint64_t* __restrict__ offs,
                  const uint64_t* __restrict__ slot_offs, uint64_t slot_base, uint64_t n_reads, unsigned k,
                  uint64_t* __restrict__ h0_out, uint8_t* __restrict__ valid_out, bool may_stage)
 {
-	__shared__ uint64_t sP[kHashWarps][kRing];
-	__shared__ uint64_t sQ[kHashWarps][kRing];
-	__shared__ unsigned sB[kHashWarps][kRing];
+	constexpr int W = ring_warps<RING>();
+	__shared__ uint64_t sP[W][RING];
+	__shared__ uint64_t sQ[W][RING];
+	__shared__ unsigned sB[W][RING];
 	extern __shared__ __align__(128) uint8_t stage_mem[]; // 2 x kTmaStage bytes (dynamic: the rings above use 40 KB of static)
 	uint8_t* const stage[2] = { stage_mem, stage_mem + kTmaStage };
 	__shared__ cuda::barrier<cuda::thread_scope_block> bar[2];
@@ -328,14 +338,14 @@ k_hash_reads_tma(const uint8_t* __restrict__ bases, const uint64_t* __restrict__
 			__syncthreads();
 		}
 		const uint64_t r_end = min(n_reads, (b + 1) * (uint64_t)kTmaReads);
-		for (uint64_t r = b * kTmaReads + warp; r < r_end; r += kHashWarps) {
+		for (uint64_t r = b * kTmaReads + warp; r < r_end; r += W) {
 			const uint64_t beg = offs[r];
 			const unsigned L = (unsigned)(offs[r + 1] - beg);
 			if (L >= k) {
 				if (staged)
-					hash_one_read(stage[st], beg - a0, L, slot_offs[r] - slot_base, k, sP[warp], sQ[warp], sB[warp], lane, h0_out, valid_out);
+					hash_one_read<RING>(stage[st], beg - a0, L, slot_offs[r] - slot_base, k, sP[warp], sQ[warp], sB[warp], lane, h0_out, valid_out);
 				else
-					hash_one_read(bases, beg, L, slot_offs[r] - slot_base, k, sP[warp], sQ[warp], sB[warp], lane, h0_out, valid_out);
+					hash_one_read<RING>(bases, beg, L, slot_offs[r] - slot_base, k, sP[warp], sQ[warp], sB[warp], lane, h0_out, valid_out);
 			}
 		}
 		__syncthreads(); // everybody is done with stage[st] before it is refilled two iterations later
@@ -346,20 +356,22 @@ k_hash_reads_tma(const uint8_t* __restrict__ bases, const uint64_t* __restrict__
 
 /** the same over explicit segments (long sequences are cut into overlapping pieces so that every
  *  warp has work): segment s = bases [seg_beg[s], +seg_len[s]), its first window is slot seg_slot[s] */
-static __global__ void __launch_bounds__(kHashWarps * 32)
+template <int RING>
+static __global__ void __launch_bounds__(ring_warps<RING>() * 32)
 k_hash_segments(const uint8_t* __restrict__ bases, const uint64_t* __restrict__ seg_beg, const unsigned* __restrict__ seg_len,
                 const uint64_t* __restrict__ seg_slot, uint64_t n_segs, unsigned k, uint64_t* __restrict__ h0_out,
                 uint8_t* __restrict__ valid_out)
 {
-	__shared__ uint64_t sP[kHashWarps][kRing];
-	__shared__ uint64_t sQ[kHashWarps][kRing];
-	__shared__ unsigned sB[kHashWarps][kRing];
+	constexpr int W = ring_warps<RING>();
+	__shared__ uint64_t sP[W][RING];
+	__shared__ uint64_t sQ[W][RING];
+	__shared__ unsigned sB[W][RING];
 	const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-	for (uint64_t r = (uint64_t)blockIdx.x * kHashWarps + warp; r < n_segs; r += (uint64_t)gridDim.x * kHashWarps) {
+	for (uint64_t r = (uint64_t)blockIdx.x * W + warp; r < n_segs; r += (uint64_t)gridDim.x * W) {
 		const unsigned L = seg_len[r];
 		if (L < k)
 			continue;
-		hash_one_read(bases, seg_beg[r], L, seg_slot[r], k, sP[warp], sQ[warp], sB[warp], lane, h0_out, valid_out);
+		hash_one_read<RING>(bases, seg_beg[r], L, seg_slot[r], k, sP[warp], sQ[warp], sB[warp], lane, h0_out, valid_out);
 	}
 }
 

@@ -41,8 +41,12 @@ int kon_insert_reads_dev(abb_filter* f, const uint8_t* d_bases, const uint64_t* 
 	unsigned long long* d_count = f->d_stats.p + kStatKonKmers;
 	ABB_CUDA(cudaMemsetAsync(d_count, 0, sizeof(unsigned long long), f->stream));
 	ABB_CUDA(cudaEventRecord(f->ev0, f->stream));
-	k_kon_walk<false><<<kon_grid(total), 256, 0, f->stream>>>(d_bases, d_offs, f->slot_offs.p, n_reads, total, kon_geom(f->k), kon_view(f),
-	                                                          nullptr, nullptr, d_count);
+	if (kon_words(f->k) == kKonWords)
+		k_kon_walk<false, kKonWords><<<kon_grid(total), 256, 0, f->stream>>>(d_bases, d_offs, f->slot_offs.p, n_reads, total, kon_geom(f->k),
+		                                                                     kon_view(f), nullptr, nullptr, d_count);
+	else
+		k_kon_walk<false, kKonWordsWide><<<kon_grid(total), 256, 0, f->stream>>>(d_bases, d_offs, f->slot_offs.p, n_reads, total,
+		                                                                         kon_geom(f->k), kon_view(f), nullptr, nullptr, d_count);
 	ABB_CUDA(cudaGetLastError());
 	ABB_CUDA(cudaEventRecord(f->ev1, f->stream));
 	unsigned long long n = 0;
@@ -61,8 +65,12 @@ int kon_insert_reads_dev(abb_filter* f, const uint8_t* d_bases, const uint64_t* 
 
 int kon_query_slots(abb_filter* f, const uint8_t* d_bases, const uint64_t* d_offs, uint64_t n_reads, uint64_t n_slots)
 {
-	k_kon_walk<true><<<kon_grid(n_slots), 256, 0, f->stream>>>(d_bases, d_offs, f->slot_offs.p, n_reads, n_slots, kon_geom(f->k), kon_view(f),
-	                                                           f->out8.p, f->valid.p, nullptr);
+	if (kon_words(f->k) == kKonWords)
+		k_kon_walk<true, kKonWords><<<kon_grid(n_slots), 256, 0, f->stream>>>(d_bases, d_offs, f->slot_offs.p, n_reads, n_slots, kon_geom(f->k),
+		                                                                      kon_view(f), f->out8.p, f->valid.p, nullptr);
+	else
+		k_kon_walk<true, kKonWordsWide><<<kon_grid(n_slots), 256, 0, f->stream>>>(d_bases, d_offs, f->slot_offs.p, n_reads, n_slots,
+		                                                                          kon_geom(f->k), kon_view(f), f->out8.p, f->valid.p, nullptr);
 	f->st.launches += 1;
 	ABB_CUDA(cudaGetLastError());
 	return ABB_OK;
@@ -134,8 +142,12 @@ int abb_trim_reads(abb_filter* f, const char* bases, const uint64_t* offsets, ui
 	for (uint64_t r = 0; r < n_reads; ++r)
 		ABB_REQUIRE(offsets[r + 1] - offsets[r] < (1ULL << 31), "read %llu is too long", (unsigned long long)r);
 	ABB_CUDA(cudaSetDevice(f->device));
+	const bool wide = kon_words(f->k) != kKonWords;
 	int per_sm = 0; // a grid that is resident all at once: the walk scratch is sized per warp of the grid
-	ABB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_kon_trim, kKonTrimThreads, 0));
+	if (wide)
+		ABB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_kon_trim<kKonWordsWide>, kKonTrimThreads, 0));
+	else
+		ABB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_kon_trim<kKonWords>, kKonTrimThreads, 0));
 	const unsigned blocks =
 	    (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(blocks_for(2 * n_reads * 32, kKonTrimThreads), (uint64_t)sm_count() * std::max(per_sm, 1)));
 	const uint64_t n_warps = (uint64_t)blocks * kKonTrimThreads / 32;
@@ -149,8 +161,12 @@ int abb_trim_reads(abb_filter* f, const char* bases, const uint64_t* offsets, ui
 	uint64_t* d_look = reinterpret_cast<uint64_t*>(f->trim_scratch.p + frame_bytes);
 	const SyncOnExit sync = { f->stream };
 	ABB_CHECK(stage_read_batch(bases, offsets, n_reads, d_bases, d_offs, f->stream));
-	k_kon_trim<<<blocks, kKonTrimThreads, 0, f->stream>>>(d_bases.p, d_offs.p, n_reads, kon_geom(f->k), kon_view(f), min_branch_len, d_frames,
-	                                                      d_look, d_out.p, d_out.p + n_reads);
+	if (wide)
+		k_kon_trim<kKonWordsWide><<<blocks, kKonTrimThreads, 0, f->stream>>>(d_bases.p, d_offs.p, n_reads, kon_geom(f->k), kon_view(f),
+		                                                                     min_branch_len, d_frames, d_look, d_out.p, d_out.p + n_reads);
+	else
+		k_kon_trim<kKonWords><<<blocks, kKonTrimThreads, 0, f->stream>>>(d_bases.p, d_offs.p, n_reads, kon_geom(f->k), kon_view(f),
+		                                                                 min_branch_len, d_frames, d_look, d_out.p, d_out.p + n_reads);
 	ABB_CUDA(cudaGetLastError());
 	f->st.launches += 1;
 	ABB_CUDA(cudaMemcpyAsync(left, d_out.p, n_reads * sizeof(uint32_t), cudaMemcpyDeviceToHost, f->stream));

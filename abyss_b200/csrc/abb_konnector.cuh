@@ -4,15 +4,18 @@
 // tests/host_konnector runs the same arithmetic against the reference's files.
 //
 // K-mer bytes (Common/Kmer.cpp): A0 C1 G2 T3, base i in byte i/4 at bits 2*(3 - i%4), padding zero, (k+3)/4 bytes.  Here a
-// k-mer is held as up to six big-endian 64-bit words (base i at bit 62 - 2*(i%32) of word i/32), so byte j of the packed
-// k-mer is byte 7 - j%8 of word j/8 and the byte string CityHash reads is the words' big-endian image.
+// k-mer is held as NW big-endian 64-bit words (base i at bit 62 - 2*(i%32) of word i/32), so byte j of the packed k-mer is
+// byte 7 - j%8 of word j/8 and the byte string CityHash reads is the words' big-endian image.  NW is 6 for k <= 192 and 8
+// for k = 193..256 (kon_words), one kernel instance per width, so that k <= 192 does not carry two more words per image.
 #pragma once
 #include "abb_device.cuh"
 #include "abb_walk.cuh"
 
 namespace abb {
 
-constexpr unsigned kKonWords = 6; // 2 * kMaxK bits
+constexpr unsigned kKonWords = 6;     // words of a k-mer up to k = 192
+constexpr unsigned kKonWordsWide = 8; // k = 193..kMaxK
+inline unsigned kon_words(unsigned k) { return k <= 32 * kKonWords ? kKonWords : kKonWordsWide; }
 
 #if defined(__CUDA_ARCH__)
 #define KON_UNROLL _Pragma("unroll")
@@ -20,7 +23,7 @@ constexpr unsigned kKonWords = 6; // 2 * kMaxK bits
 #define KON_UNROLL
 #endif
 
-// ---- CityHash64WithSeed (CityHash 1.0, Geoff Pike and Jyrki Alakuijala), inputs of 1..48 bytes ------------------------
+// ---- CityHash64WithSeed (CityHash 1.0, Geoff Pike and Jyrki Alakuijala), inputs of 1..64 bytes ------------------------
 constexpr uint64_t kCityK0 = 0xc3a5c85c97cb3127ULL;
 constexpr uint64_t kCityK1 = 0xb492b66fbe98f273ULL;
 constexpr uint64_t kCityK2 = 0x9ae16a3b2f90404fULL;
@@ -49,78 +52,86 @@ ABB_HD uint64_t city_hash16(uint64_t lo, uint64_t hi)
 }
 
 /** word i of a k-mer image, 0 past the end (a select chain keeps the words in registers) */
+template <unsigned NW>
 ABB_HD uint64_t kon_word(const uint64_t* w, unsigned i)
 {
 	uint64_t r = 0;
 KON_UNROLL
-	for (unsigned j = 0; j < kKonWords; ++j)
+	for (unsigned j = 0; j < NW; ++j)
 		r = j == i ? w[j] : r;
 	return r;
 }
 /** little-endian 64-bit load at byte offset o of the big-endian word image */
+template <unsigned NW>
 ABB_HD uint64_t kon_fetch64(const uint64_t* w, unsigned o)
 {
 	const unsigned s = 8 * (o % 8);
-	const uint64_t hi = kon_word(w, o / 8), lo = kon_word(w, o / 8 + 1);
+	const uint64_t hi = kon_word<NW>(w, o / 8), lo = kon_word<NW>(w, o / 8 + 1);
 	return city_bswap64(s ? (hi << s) | (lo >> (64 - s)) : hi);
 }
-ABB_HD uint64_t kon_fetch32(const uint64_t* w, unsigned o) { return kon_fetch64(w, o) & 0xffffffffULL; }
-ABB_HD unsigned kon_byte(const uint64_t* w, unsigned o) { return (unsigned)(kon_word(w, o / 8) >> (56 - 8 * (o % 8))) & 0xffu; }
+template <unsigned NW>
+ABB_HD uint64_t kon_fetch32(const uint64_t* w, unsigned o) { return kon_fetch64<NW>(w, o) & 0xffffffffULL; }
+template <unsigned NW>
+ABB_HD unsigned kon_byte(const uint64_t* w, unsigned o) { return (unsigned)(kon_word<NW>(w, o / 8) >> (56 - 8 * (o % 8))) & 0xffu; }
 
-/** CityHash64 of the first len (1..48) bytes of the image */
+/** CityHash64 of the first len (1..8 * NW, at most 64) bytes of an image of NW words */
+template <unsigned NW>
 ABB_HD uint64_t city64(const uint64_t* w, unsigned len)
 {
 	if (len > 32) { // 33..64 bytes
-		uint64_t z = kon_fetch64(w, 24);
-		uint64_t a = kon_fetch64(w, 0) + (len + kon_fetch64(w, len - 16)) * kCityK0;
+		uint64_t z = kon_fetch64<NW>(w, 24);
+		uint64_t a = kon_fetch64<NW>(w, 0) + (len + kon_fetch64<NW>(w, len - 16)) * kCityK0;
 		uint64_t b = city_rot(a + z, 52);
 		uint64_t c = city_rot(a, 37);
-		a += kon_fetch64(w, 8);
+		a += kon_fetch64<NW>(w, 8);
 		c += city_rot(a, 7);
-		a += kon_fetch64(w, 16);
+		a += kon_fetch64<NW>(w, 16);
 		const uint64_t vf = a + z, vs = b + city_rot(a, 31) + c;
-		a = kon_fetch64(w, 16) + kon_fetch64(w, len - 32);
-		z = kon_fetch64(w, len - 8);
+		a = kon_fetch64<NW>(w, 16) + kon_fetch64<NW>(w, len - 32);
+		z = kon_fetch64<NW>(w, len - 8);
 		b = city_rot(a + z, 52);
 		c = city_rot(a, 37);
-		a += kon_fetch64(w, len - 24);
+		a += kon_fetch64<NW>(w, len - 24);
 		c += city_rot(a, 7);
-		a += kon_fetch64(w, len - 16);
+		a += kon_fetch64<NW>(w, len - 16);
 		const uint64_t wf = a + z, ws = b + city_rot(a, 31) + c;
 		const uint64_t r = city_shift_mix((vf + ws) * kCityK2 + (wf + vs) * kCityK0);
 		return city_shift_mix(r * kCityK0 + vs) * kCityK2;
 	}
 	if (len > 16) { // 17..32 bytes
-		const uint64_t a = kon_fetch64(w, 0) * kCityK1, b = kon_fetch64(w, 8);
-		const uint64_t c = kon_fetch64(w, len - 8) * kCityK2, d = kon_fetch64(w, len - 16) * kCityK0;
+		const uint64_t a = kon_fetch64<NW>(w, 0) * kCityK1, b = kon_fetch64<NW>(w, 8);
+		const uint64_t c = kon_fetch64<NW>(w, len - 8) * kCityK2, d = kon_fetch64<NW>(w, len - 16) * kCityK0;
 		return city_hash16(city_rot(a - b, 43) + city_rot(c, 30) + d, a + city_rot(b ^ kCityK3, 20) - c + len);
 	}
 	if (len > 8) {
-		const uint64_t a = kon_fetch64(w, 0), b = kon_fetch64(w, len - 8);
+		const uint64_t a = kon_fetch64<NW>(w, 0), b = kon_fetch64<NW>(w, len - 8);
 		return city_hash16(a, city_rot(b + len, len)) ^ b;
 	}
 	if (len >= 4) {
-		const uint64_t a = kon_fetch32(w, 0);
-		return city_hash16(len + (a << 3), kon_fetch32(w, len - 4));
+		const uint64_t a = kon_fetch32<NW>(w, 0);
+		return city_hash16(len + (a << 3), kon_fetch32<NW>(w, len - 4));
 	}
-	const uint32_t y = kon_byte(w, 0) + ((uint32_t)kon_byte(w, len >> 1) << 8);
-	const uint32_t z = len + ((uint32_t)kon_byte(w, len - 1) << 2);
+	const uint32_t y = kon_byte<NW>(w, 0) + ((uint32_t)kon_byte<NW>(w, len >> 1) << 8);
+	const uint32_t z = len + ((uint32_t)kon_byte<NW>(w, len - 1) << 2);
 	return city_shift_mix(y * kCityK2 ^ z * kCityK3) * kCityK2;
 }
 
 /** Bloom::hash(kmer, seed) (Bloom/Bloom.h:63-71): CityHash64WithSeed of the canonical k-mer's (k+3)/4 bytes */
+template <unsigned NW>
 ABB_HD uint64_t city64_seed(const uint64_t* w, unsigned len, uint64_t seed)
 {
-	return city_hash16(city64(w, len) - kCityK2, seed);
+	return city_hash16(city64<NW>(w, len) - kCityK2, seed);
 }
 
 // ---- the rolling canonical k-mer ---------------------------------------------------------------------------------------
 /** forward and reverse-complement images of the current window, rolled one base at a time; `run` counts the ACGT bases
  *  since the last other character, so the window is a k-mer exactly when run >= k (Bloom::loadSeq skips the others) */
-struct KonKmer {
-	uint64_t f[kKonWords], r[kKonWords];
+template <unsigned NW>
+struct KonKmerN {
+	uint64_t f[NW], r[NW];
 	unsigned run;
 };
+using KonKmer = KonKmerN<kKonWords>;
 
 struct KonGeom {
 	unsigned k, nbytes;       // k, (k+3)/4
@@ -140,16 +151,18 @@ inline KonGeom kon_geom(unsigned k) // host only
 	return g;
 }
 
-ABB_HD void kon_clear(KonKmer& m)
+template <unsigned NW>
+ABB_HD void kon_clear(KonKmerN<NW>& m)
 {
 KON_UNROLL
-	for (unsigned j = 0; j < kKonWords; ++j)
+	for (unsigned j = 0; j < NW; ++j)
 		m.f[j] = m.r[j] = 0;
 	m.run = 0;
 }
 
 /** append character c (any case) to the window */
-ABB_HD void kon_push(KonKmer& m, const KonGeom& g, unsigned char c)
+template <unsigned NW>
+ABB_HD void kon_push(KonKmerN<NW>& m, const KonGeom& g, unsigned char c)
 {
 	unsigned code = base_code(c);
 	if (code > 3) {
@@ -158,38 +171,39 @@ ABB_HD void kon_push(KonKmer& m, const KonGeom& g, unsigned char c)
 	} else
 		++m.run;
 KON_UNROLL
-	for (unsigned j = 0; j < kKonWords; ++j) // forward: shift left one base, the new base goes to position k-1
-		m.f[j] = (m.f[j] << 2) | (j + 1 < kKonWords ? m.f[j + 1] >> 62 : 0);
+	for (unsigned j = 0; j < NW; ++j) // forward: shift left one base, the new base goes to position k-1
+		m.f[j] = (m.f[j] << 2) | (j + 1 < NW ? m.f[j + 1] >> 62 : 0);
 KON_UNROLL
-	for (int j = kKonWords - 1; j >= 0; --j) // reverse complement: shift right one base, the complement goes to position 0
+	for (int j = NW - 1; j >= 0; --j) // reverse complement: shift right one base, the complement goes to position 0
 		m.r[j] = (m.r[j] >> 2) | (j > 0 ? m.r[j - 1] << 62 : 0);
 	m.r[0] |= (uint64_t)(3 - code) << 62;
 KON_UNROLL
-	for (unsigned j = 0; j < kKonWords; ++j) {
+	for (unsigned j = 0; j < NW; ++j) {
 		const uint64_t keep = j < g.last_word ? ~0ULL : j == g.last_word ? g.last_mask : 0ULL;
 		m.f[j] &= keep;
 		m.r[j] &= keep;
 	}
 KON_UNROLL
-	for (unsigned j = 0; j < kKonWords; ++j)
+	for (unsigned j = 0; j < NW; ++j)
 		if (j == g.last_word)
 			m.f[j] |= (uint64_t)code << g.last_shift;
 }
 
 /** Bloom::hash of the current window: the forward image when it is not larger than its reverse complement
  *  (Kmer::isCanonical, Common/Kmer.cpp:297-310), else the reverse complement */
-ABB_HD uint64_t kon_hash(const KonKmer& m, const KonGeom& g, uint64_t seed)
+template <unsigned NW>
+ABB_HD uint64_t kon_hash(const KonKmerN<NW>& m, const KonGeom& g, uint64_t seed)
 {
 	int cmp = 0;
 KON_UNROLL
-	for (unsigned j = 0; j < kKonWords; ++j)
+	for (unsigned j = 0; j < NW; ++j)
 		if (cmp == 0 && m.f[j] != m.r[j])
 			cmp = m.f[j] < m.r[j] ? -1 : 1;
-	uint64_t c[kKonWords];
+	uint64_t c[NW];
 KON_UNROLL
-	for (unsigned j = 0; j < kKonWords; ++j)
+	for (unsigned j = 0; j < NW; ++j)
 		c[j] = cmp <= 0 ? m.f[j] : m.r[j];
-	return city64_seed(c, g.nbytes, seed);
+	return city64_seed<NW>(c, g.nbytes, seed);
 }
 
 // ---- filter geometry ---------------------------------------------------------------------------------------------------
@@ -279,12 +293,13 @@ ABB_HD uint8_t kon_copy_bits_byte(uint8_t old, const uint8_t* src, uint64_t bits
 /** One step of a k-mer in place: FWD drops base 0 and appends b (Kmer::shift(SENSE) + setLastBase), REV drops base k-1 and
  *  prepends b; both images follow.  A step to the left of the forward image is a step to the right of the reverse
  *  complement with the complementary base, so one shift serves both directions.  Only the words that k uses are shifted:
- *  a step sits on the critical path of every graph move, where kon_push (a bulk scan) shifts all six. */
-ABB_HD void kon_step(KonKmer& m, const KonGeom& g, Dir d, unsigned b)
+ *  a step sits on the critical path of every graph move, where kon_push (a bulk scan) shifts all NW. */
+template <unsigned NW>
+ABB_HD void kon_step(KonKmerN<NW>& m, const KonGeom& g, Dir d, unsigned b)
 {
 	if (d == REV) {
 KON_UNROLL
-		for (unsigned j = 0; j < kKonWords; ++j) {
+		for (unsigned j = 0; j < NW; ++j) {
 			const uint64_t t = m.f[j];
 			m.f[j] = m.r[j];
 			m.r[j] = t;
@@ -292,15 +307,15 @@ KON_UNROLL
 		b = 3 - b;
 	}
 KON_UNROLL
-	for (unsigned j = 0; j < kKonWords; ++j) { // shift left one base, b goes to position k-1
+	for (unsigned j = 0; j < NW; ++j) { // shift left one base, b goes to position k-1
 		if (j > g.last_word)
 			break;
-		m.f[j] = (m.f[j] << 2) | (j + 1 < kKonWords && j < g.last_word ? m.f[j + 1 < kKonWords ? j + 1 : j] >> 62 : 0);
+		m.f[j] = (m.f[j] << 2) | (j + 1 < NW && j < g.last_word ? m.f[j + 1 < NW ? j + 1 : j] >> 62 : 0);
 		if (j == g.last_word)
 			m.f[j] |= (uint64_t)b << g.last_shift;
 	}
 KON_UNROLL
-	for (int j = kKonWords - 1; j >= 0; --j) { // shift right one base, the complement goes to position 0
+	for (int j = NW - 1; j >= 0; --j) { // shift right one base, the complement goes to position 0
 		if ((unsigned)j > g.last_word)
 			continue;
 		m.r[j] = (m.r[j] >> 2) | (j > 0 ? m.r[j > 0 ? j - 1 : 0] << 62 : 0);
@@ -310,7 +325,7 @@ KON_UNROLL
 	m.r[0] |= (uint64_t)(3 - b) << 62;
 	if (d == REV) {
 KON_UNROLL
-		for (unsigned j = 0; j < kKonWords; ++j) {
+		for (unsigned j = 0; j < NW; ++j) {
 			const uint64_t t = m.f[j];
 			m.f[j] = m.r[j];
 			m.r[j] = t;
@@ -324,16 +339,19 @@ KON_UNROLL
  *  (exact), a chain of CityHash's 128-to-64-bit mix over its words above that.  A walk compares a vertex with at most
  *  kFrameCap + kLookCap others, all within a few dozen steps of one read k-mer; two different k-mers among them sharing
  *  the 64-bit mix is a ~2^-64 event per comparison, the same order as the ntHash identity of the pass-2 walk. */
-struct KonVtx {
-	KonKmer m;
+template <unsigned NW>
+struct KonVtxN {
+	KonKmerN<NW> m;
 	uint64_t id;
 	ABB_HD uint64_t canon() const { return id; }
 };
-ABB_HD uint64_t kon_identity(const KonKmer& m, const KonGeom& g)
+using KonVtx = KonVtxN<kKonWords>;
+template <unsigned NW>
+ABB_HD uint64_t kon_identity(const KonKmerN<NW>& m, const KonGeom& g)
 {
 	uint64_t id = m.f[0];
 KON_UNROLL
-	for (unsigned j = 1; j < kKonWords; ++j) {
+	for (unsigned j = 1; j < NW; ++j) {
 		if (j > g.last_word)
 			break;
 		id = city_hash16(id, m.f[j]);
@@ -341,20 +359,23 @@ KON_UNROLL
 	return id;
 }
 /** the vertex interface of the walk templates (abb_walk.cuh); returns the base that fell off */
-ABB_HD unsigned vtx_step(KonVtx& v, unsigned, const KonGeom& g, Dir d, unsigned b)
+template <unsigned NW>
+ABB_HD unsigned vtx_step(KonVtxN<NW>& v, unsigned, const KonGeom& g, Dir d, unsigned b)
 {
 	const unsigned out = d == FWD ? (unsigned)(v.m.f[0] >> 62) : 3u - (unsigned)(v.m.r[0] >> 62);
 	kon_step(v.m, g, d, b);
 	v.id = kon_identity(v.m, g);
 	return out;
 }
-ABB_HD void vtx_unstep(KonVtx& v, unsigned k, const KonGeom& g, Dir d, unsigned out) { vtx_step(v, k, g, opposite(d), out); }
+template <unsigned NW>
+ABB_HD void vtx_unstep(KonVtxN<NW>& v, unsigned k, const KonGeom& g, Dir d, unsigned out) { vtx_step(v, k, g, opposite(d), out); }
 
 /** Bloom::hash of neighbour n of m: n = 0..3 the out-edges (append A, C, G, T: out_edge_iterator, DBGBloom.h:160-221),
  *  4..7 the in-edges (prepend A, C, G, T: in_edge_iterator, :224-285), 8 the k-mer itself */
-ABB_HD uint64_t kon_neighbor_hash(const KonKmer& m, const KonGeom& g, uint64_t seed, unsigned n)
+template <unsigned NW>
+ABB_HD uint64_t kon_neighbor_hash(const KonKmerN<NW>& m, const KonGeom& g, uint64_t seed, unsigned n)
 {
-	KonKmer t = m;
+	KonKmerN<NW> t = m;
 	if (n < 8)
 		kon_step(t, g, n < 4 ? FWD : REV, n & 3);
 	return kon_hash(t, g, seed);
@@ -381,15 +402,15 @@ constexpr uint32_t kKonTrimFailed = 0xffffffffu; // the walk scratch overflowed:
  *
  * Ctx is the walk context of abb_walk.cuh (k, trim = minBranchLen, rt = the KonGeom, neighbors / neighbors_dir, the scratch
  * accessors) plus
- *   unsigned neighbors_self(const KonVtx&)   neighbors() with bit 8 = the k-mer itself is in the filter: nine probes issued
+ *   unsigned neighbors_self(const KonVtxN<NW>&)   neighbors() with bit 8 = the k-mer itself is in the filter: nine probes issued
  *                                            together, so a window costs one memory round trip whether or not it is a vertex
  *   unsigned char base(const uint8_t* seq, unsigned len, unsigned i)   seq[i]
  */
-template <class Ctx>
+template <unsigned NW = kKonWords, class Ctx>
 ABB_HD uint32_t kon_left_trim(Ctx& c, const uint8_t* seq, unsigned len, bool rc)
 {
 	const unsigned k = c.k;
-	KonVtx v;
+	KonVtxN<NW> v;
 	kon_clear(v.m);
 	unsigned run = 0;
 	bool first = true;
@@ -449,7 +470,7 @@ __device__ __forceinline__ uint64_t kon_read_of(const uint64_t* __restrict__ slo
  *     dropped (BloomFilterWindow::insert).
  *   kQuery = true: writes the bit of the last level to flag[slot] and the window's validity to valid[slot].
  *  n_kmers (optional) counts the valid windows. */
-template <bool kQuery>
+template <bool kQuery, unsigned NW>
 __global__ void __launch_bounds__(256) k_kon_walk(const uint8_t* __restrict__ bases, const uint64_t* __restrict__ offs,
                                                   const uint64_t* __restrict__ slot_offs, uint64_t n_reads, uint64_t n_slots,
                                                   KonGeom g, KonView fv, uint8_t* __restrict__ flag, uint8_t* __restrict__ valid,
@@ -467,7 +488,7 @@ __global__ void __launch_bounds__(256) k_kon_walk(const uint8_t* __restrict__ ba
 			const uint64_t read_end = min(s1, slot_offs[r + 1]);
 			const uint8_t* seq = bases + offs[r];
 			const uint64_t p0 = s - slot_offs[r]; // first window of this read handled here
-			KonKmer m;
+			KonKmerN<NW> m;
 			kon_clear(m);
 			for (unsigned i = 0; i + 1 < g.k; ++i)
 				kon_push(m, g, seq[p0 + i]);
@@ -568,6 +589,7 @@ __global__ void k_kon_compare(const uint8_t* __restrict__ a, const uint8_t* __re
  *  only in the probes, where lane n < 9 hashes neighbour n (kon_neighbor_hash) and loads its bit, and in the scratch
  *  accessors.  The scratch conventions are WarpCtx's (abb_assemble.cu): every lane stores the same value and reads back
  *  its own store. */
+template <unsigned NW>
 struct KonWarpCtx {
 	unsigned k, trim;
 	KonGeom rt;
@@ -579,16 +601,16 @@ struct KonWarpCtx {
 	unsigned chunk;       // which 32 characters of the read `held` is
 	unsigned char held;   // character 32 * chunk + lane
 
-	__device__ unsigned probe(const KonVtx& v, unsigned lanes) const
+	__device__ unsigned probe(const KonVtxN<NW>& v, unsigned lanes) const
 	{
 		bool ok = false;
 		if ((lanes >> lane) & 1u)
 			ok = kon_test(fv, kon_neighbor_hash(v.m, rt, fv.seed, lane));
 		return __ballot_sync(0xffffffffu, ok);
 	}
-	__device__ unsigned neighbors_self(const KonVtx& v) const { return probe(v, 0x1ffu); }
-	__device__ unsigned neighbors(const KonVtx& v) const { return probe(v, 0xffu); }
-	__device__ unsigned neighbors_dir(const KonVtx& v, Dir d) const { return d == FWD ? probe(v, 0x0fu) : probe(v, 0xf0u) >> 4; }
+	__device__ unsigned neighbors_self(const KonVtxN<NW>& v) const { return probe(v, 0x1ffu); }
+	__device__ unsigned neighbors(const KonVtxN<NW>& v) const { return probe(v, 0xffu); }
+	__device__ unsigned neighbors_dir(const KonVtxN<NW>& v, Dir d) const { return d == FWD ? probe(v, 0x0fu) : probe(v, 0xf0u) >> 4; }
 	/** seq[i]: the warp keeps 32 characters in registers (one coalesced load per 32 windows instead of one load per window) */
 	__device__ unsigned char base(const uint8_t* seq, unsigned len, unsigned i)
 	{
@@ -624,13 +646,14 @@ constexpr unsigned kKonTrimThreads = 128;
  *  end at their first window after one probe round, a few walk tens of windows with a trueBranch search at each, and with
  *  hundreds of tasks per warp, the two ends of a read and neighbouring reads on different warps, the long ones spread out.
  *  frames / look: kFrameCap / kLookCap entries per warp of the grid. */
+template <unsigned NW>
 __global__ void __launch_bounds__(kKonTrimThreads) k_kon_trim(const uint8_t* __restrict__ bases, const uint64_t* __restrict__ offs,
                                                              uint64_t n_reads, KonGeom g, KonView fv, unsigned min_branch_len,
                                                              Frame* __restrict__ frames, uint64_t* __restrict__ look,
                                                              uint32_t* __restrict__ left, uint32_t* __restrict__ right)
 {
 	const uint64_t warp = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) / 32, n_warps = (uint64_t)gridDim.x * blockDim.x / 32;
-	KonWarpCtx c;
+	KonWarpCtx<NW> c;
 	c.k = g.k;
 	c.trim = min_branch_len;
 	c.rt = g;
@@ -644,7 +667,7 @@ __global__ void __launch_bounds__(kKonTrimThreads) k_kon_trim(const uint8_t* __r
 		if (len >= g.k) {
 			c.fail_ = 0;
 			c.chunk = 0xffffffffu;
-			out = kon_left_trim(c, bases + b0, (unsigned)len, (t & 1) != 0);
+			out = kon_left_trim<NW>(c, bases + b0, (unsigned)len, (t & 1) != 0);
 		}
 		if (c.lane == 0)
 			(t & 1 ? right : left)[r] = out;

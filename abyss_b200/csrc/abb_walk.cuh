@@ -855,7 +855,7 @@ ABB_HD Vtx<KW> rebuild_head(Ctx& c, const Vtx<KW>& start, const ByteVec& v, unsi
 	const unsigned pushed = v.n - from;
 	if (pushed >= k) {
 		// the last k pushed bases spell the vertex (REV pushes prepend: newest base first)
-		uint8_t tmp[kMaxK];
+		uint8_t tmp[KW > 6 ? 32 * KW : 192]; // the k bases; 192 bytes up to six words keeps those instances' stack frames
 		for (unsigned i = 0; i < k; ++i)
 			tmp[i] = d == FWD ? c.rd8(v.p + v.n - k + i) : c.rd8(v.p + v.n - 1 - i);
 		return vtx_from_codes<KW>(tmp, k, false, c.rt);

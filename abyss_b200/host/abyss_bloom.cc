@@ -16,6 +16,7 @@
 #include "../../include/abyss_b200.h"
 #include "bloom_file.h"
 #include "bloom_graph.h"
+#include "max_kmer.h"
 #include "reads.h"
 #include "trim.h"
 #include <getopt.h>
@@ -782,6 +783,7 @@ static int graph(int argc, char** argv)
 
 int main(int argc, char** argv)
 {
+	apply_max_kmer(PROGRAM);
 	const std::string cmd = argc >= 2 ? argv[1] : "";
 	if (cmd == "info") { // the first operand once getopt has skipped the options (and their arguments)
 		optind = 2;

@@ -13,6 +13,7 @@
 #include "../../include/abyss_b200.h"
 #include "bloom_file.h"
 #include "graph_dump.h"
+#include "max_kmer.h"
 #include "reads.h"
 #include <getopt.h>
 #include <climits>
@@ -26,7 +27,6 @@
 #include <unordered_set>
 
 #define PROGRAM "abyss-bloom-dbg"
-#define MAX_KMER 192
 #define MAX_HASHES 32
 
 using namespace host;
@@ -308,6 +308,7 @@ static void outputGraph(const std::vector<std::string>& files, abb_filter* bloom
 
 int main(int argc, char** argv)
 {
+	const unsigned maxKmer = apply_max_kmer(PROGRAM);
 	bool die = false;
 	for (int c; (c = getopt_long(argc, argv, shortopts, longopts, NULL)) != -1;) {
 		std::istringstream arg(optarg != NULL ? optarg : "");
@@ -336,7 +337,13 @@ int main(int argc, char** argv)
 		case 'T': arg >> params.tracePath; break;
 		case 'Q': arg >> ropt.internalQThreshold; break;
 		case 'v': ++params.verbose; break;
-		case OPT_HELP: std::cout << USAGE_MESSAGE; exit(EXIT_SUCCESS);
+		case OPT_HELP: {
+			std::string usage = USAGE_MESSAGE; // `-k`'s bound is the MAX_KMER in force (ABYSS_MAX_KMER)
+			const std::string bound = "[<=192]";
+			usage.replace(usage.find(bound), bound.size(), "[<=" + std::to_string(maxKmer) + "]");
+			std::cout << usage;
+			exit(EXIT_SUCCESS);
+		}
 		case MIN_KMER_COV: arg >> params.minCov; break;
 		case OPT_VERSION: std::cout << VERSION_MESSAGE; exit(EXIT_SUCCESS);
 		case QR_SEED: params.resetSpacedSeedParams(); arg >> params.qrSeedLen; break;
@@ -373,8 +380,8 @@ int main(int argc, char** argv)
 		std::cerr << PROGRAM ": number of hash functions (`-H`) must be <= " << MAX_HASHES << "\n";
 		die = true;
 	}
-	if (params.k > MAX_KMER) {
-		std::cerr << PROGRAM ": k-mer size (`-k`) must be <= " << MAX_KMER << "\n";
+	if (params.k > maxKmer) {
+		std::cerr << PROGRAM ": k-mer size (`-k`) must be <= " << maxKmer << "\n";
 		die = true;
 	}
 	if (params.k > 0 && params.qrSeedLen > 0 && (params.qrSeedLen < 11 || params.qrSeedLen > params.k / 2)) {

@@ -52,6 +52,11 @@ typedef struct abb_assembler abb_assembler;
 int abb_version(void);
 const char* abb_last_error(void);
 int abb_device_count(void); /* <0 on error */
+/* MAX_KMER: the largest k that abb_filter_create, abb_konnector_create and abb_hash_reads accept, for the whole process.
+ * 192 by default, the reference's default (configure.ac --enable-maxk); abb_set_max_kmer sets it to any value up to 256,
+ * as the reference rebuilt with --enable-maxk=256 accepts k up to 256.  ABB_EINVAL above 256 or at 0. */
+int abb_set_max_kmer(unsigned max_k);
+unsigned abb_max_kmer(void);
 
 /* ---- filter lifecycle --------------------------------------------------------------------
  * size: number of counters (ABB_COUNTING; CountingBloomFilter ctor :31-50 pads to a multiple of

@@ -471,6 +471,24 @@ class Assembler:
         bases, offs = seqs_or_arrays if isinstance(seqs_or_arrays, tuple) else pack_reads(seqs_or_arrays)
         return self._run(self._lib.abb_assembler_process_reads, _ptr(bases), _ptr(offs), len(offs) - 1)
 
+    def assemble(self, read_ids, seqs_or_arrays, batch_reads: int | None = None):
+        """the reads in batches of `batch_reads` (all at once by default): (FASTA text as abyss-bloom-dbg prints it,
+        `>ID LEN COV read:READID` with IDs counted across batches, and the --read-log code of every read)"""
+        bases, offs = seqs_or_arrays if isinstance(seqs_or_arrays, tuple) else pack_reads(seqs_or_arrays)
+        n = len(offs) - 1
+        out, codes = [], []
+        cid = 0
+        step = batch_reads or n or 1
+        for lo in range(0, n, step):
+            hi = min(n, lo + step)
+            b0, b1 = int(offs[lo]), int(offs[hi])
+            sub = (bases[b0:b1], (offs[lo:hi + 1] - offs[lo]).astype(np.uint64))
+            for seed, seq, cov in self.process_reads(sub):
+                out.append(f">{cid} {len(seq)} {cov} read:{read_ids[seed]}\n{seq}\n")
+                cid += 1
+            codes.append(self.read_results())
+        return "".join(out), (np.concatenate(codes) if codes else np.zeros(0, dtype=np.uint8))
+
     def process_reads_dev(self, d_bases_ptr: int, d_offs_ptr: int, n_reads: int):
         return self._run(self._lib.abb_assembler_process_reads_dev, _vp(d_bases_ptr), _vp(d_offs_ptr), n_reads)
 
@@ -568,25 +586,14 @@ def bloom_dbg(read_ids, seqs_or_arrays, k: int, kc: int = 2, num_hashes: int = 4
     Returns (fasta_text, read_codes)."""
     if counters is None:
         counters = counters_for_budget(bloom_size)
-    bases, offs = seqs_or_arrays if isinstance(seqs_or_arrays, tuple) else pack_reads(seqs_or_arrays)
-    n = len(offs) - 1
+    reads = seqs_or_arrays if isinstance(seqs_or_arrays, tuple) else pack_reads(seqs_or_arrays)
     f = Filter.counting(counters, num_hashes, k, kc, mask=mask, device=device)
-    f.insert_reads((bases, offs))
+    f.insert_reads(reads)
     a = Assembler(f, trim, read_log)
-    out, codes = [], []
-    cid = 0
-    step = batch_reads or n or 1
-    for lo in range(0, n, step):
-        hi = min(n, lo + step)
-        b0, b1 = int(offs[lo]), int(offs[hi])
-        sub = (bases[b0:b1], (offs[lo:hi + 1] - offs[lo]).astype(np.uint64))
-        for seed, seq, cov in a.process_reads(sub):
-            out.append(f">{cid} {len(seq)} {cov} read:{read_ids[seed]}\n{seq}\n")
-            cid += 1
-        codes.append(a.read_results())
+    fasta, codes = a.assemble(read_ids, reads, batch_reads)
     a.close()
     f.close()
-    return "".join(out), (np.concatenate(codes) if codes else np.zeros(0, dtype=np.uint8))
+    return fasta, codes
 
 
 def overlap_graph(seqs_or_arrays, k: int, min_overlap: int = 50, ss: bool = False, device: int = 0):

@@ -7,6 +7,7 @@ import subprocess
 
 import pytest
 
+import parity
 from abyss_b200.synth import ReadSet
 
 pytestmark = pytest.mark.gpu
@@ -27,37 +28,24 @@ def cases(tmp_path_factory, abb):
 
 
 @pytest.mark.parametrize("name", ["e2e_g20k_k32", "e2e_g30k_k64", "e2e_g10k_k25_small"])
-def test_abyss_bloom_dbg_cli(cases, name):
-    c, fq, d = cases[name]
-    fa = str(d / (name + ".fa"))
-    log = str(d / (name + ".log"))
-    r = subprocess.run([os.path.join(BIN, "abyss-bloom-dbg"), f"-k{c['k']}", f"--kc={c['kc']}", f"-b{c['b']}", f"-H{c['H']}", "-j1",
-                        "--batch-reads=1500", f"--read-log={log}", "-o", fa, fq], capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    golden = os.path.join(ROOT, "tests", "golden")
-    assert open(fa).read() == open(os.path.join(golden, name + ".fa")).read()
-    assert open(log).read() == open(os.path.join(golden, name + ".readlog.tsv")).read()
+def test_abyss_bloom_dbg_cli(cases, tmp_path, name):
+    c, fq, _ = cases[name]
+    fasta, log, _ = parity.bloom_dbg_cli(c, fq, tmp_path, "--batch-reads=1500")
+    assert fasta == open(os.path.join(parity.GOLD, name + ".fa"), "rb").read()
+    assert log == open(os.path.join(parity.GOLD, name + ".readlog.tsv"), "rb").read()
 
 
 @pytest.mark.parametrize("name", ["e2e_g20k_k32", "e2e_g30k_k64", "e2e_g10k_k25_small"])
-def test_trace_file_identical_to_reference(cases, name):
+def test_trace_file_identical_to_reference(cases, tmp_path, name):
     # -T FILE: one ContigRecord row per contig handed to outputContig (seed k-mer, both extension lengths and result
     # codes, redundancy, contig id) -- the K4 parity channel SURVEY.md 7-9 names.  The reference leaves `length`
     # uninitialised for redundant rows; the golden generator and this test blank that cell.
     import gzip
-    c, fq, d = cases[name]
-    tr = str(d / (name + ".trace"))
-    r = subprocess.run([os.path.join(BIN, "abyss-bloom-dbg"), f"-k{c['k']}", f"--kc={c['kc']}", f"-b{c['b']}", f"-H{c['H']}", "-T", tr,
-                        "--batch-reads=1500", "-o", os.devnull, fq], capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    rows = [l.rstrip("\n").split("\t") for l in open(tr)]
-    for row in rows[1:]:
-        if row[2] == "1":
-            row[1] = "-"
-    got = "".join("\t".join(row) + "\n" for row in rows)
-    g = os.path.join(ROOT, "tests", "golden", name + ".trace.tsv")
+    c, fq, _ = cases[name]
+    _, _, trace = parity.bloom_dbg_cli(c, fq, tmp_path, "--batch-reads=1500")
+    g = os.path.join(parity.GOLD, name + ".trace.tsv")
     want = gzip.open(g + ".gz", "rt").read() if os.path.exists(g + ".gz") else open(g).read()
-    assert got == want
+    assert parity.blank_trace(trace) == want
 
 
 def test_checkpoints(cases):
@@ -170,17 +158,13 @@ def test_abyss_bloom_dbg_cli_bad_seed(cases):
 def test_coverage_track(cases, tmp_path):
     # -C FILE -R REF: the 0/1 "k-mer is solid" WIG track over a reference (writeCovTrack, bloom-dbg.h:1280-1334), one GPU query
     # per batch of reference records (abb_contains_reads); golden = the unmodified reference (make_golden_covtrack.py)
-    import sys
-    sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
     from make_golden_covtrack import ref_fasta
     c, fq, d = cases["e2e_g20k_k32"]
     rs = ReadSet.from_coverage(c["seed"], c["genome"], c["cov"], c["L"], c["err"])
     ref = str(tmp_path / "ref.fa")
     ref_fasta(rs, ref)
     wig = str(tmp_path / "cov.wig")
-    r = subprocess.run([os.path.join(BIN, "abyss-bloom-dbg"), f"-k{c['k']}", f"--kc={c['kc']}", f"-b{c['b']}", f"-H{c['H']}", "-C", wig, "-R", ref,
-                        "-o", os.devnull, fq], capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
+    parity.bloom_dbg_cli(c, fq, tmp_path, "-C", wig, "-R", ref)
     assert open(wig).read() == open(os.path.join(ROOT, "tests", "golden", "covtrack_g20k_k32.wig")).read()
     # -C without -R is a usage error, as in the reference (bloom-dbg.cc:512-515)
     r = subprocess.run([os.path.join(BIN, "abyss-bloom-dbg"), "-k32", "-b1M", "-C", wig, fq], capture_output=True, text=True)
@@ -191,22 +175,13 @@ def test_graphviz_dump(tmp_path, abb):
     # -g FILE: the breadth-first GraphViz dump of the Bloom filter de Bruijn graph (outputGraph, bloom-dbg.h:1171-1242): the
     # traversal order is the reference's, the Bloom lookups are GPU batches (abb_contains_reads, abb_successors); goldens from
     # the unmodified reference (make_golden_graph.py)
-    import gzip
-    import sys
-    sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
     from make_golden_graph import write_reads
-    for c in json.load(open(os.path.join(ROOT, "tests", "golden", "graph_cases.json"))):
+    for c in json.load(open(os.path.join(parity.GOLD, "graph_cases.json"))):
         fq = str(tmp_path / (c["name"] + ".fq"))
         write_reads(c, fq)
         dot = str(tmp_path / (c["name"] + ".dot"))
-        r = subprocess.run([os.path.join(BIN, "abyss-bloom-dbg"), f"-k{c['k']}", f"--kc={c['kc']}", f"-b{c['b']}", f"-H{c['H']}", "-g", dot,
-                            "--batch-reads=700", "-o", os.devnull, fq], capture_output=True, text=True)
-        assert r.returncode == 0, r.stderr
-        data = open(dot, "rb").read()
-        assert len(data) == c["bytes"] and hashlib.sha256(data).hexdigest() == c["sha256"], c["name"]
-        full = os.path.join(ROOT, "tests", "golden", c["name"] + ".dot.gz")
-        if os.path.exists(full):
-            assert data == gzip.open(full, "rb").read()
+        parity.bloom_dbg_cli(c, fq, tmp_path, "-g", dot, "--batch-reads=700")
+        parity.check_dump(open(dot, "rb").read(), c, os.path.join(parity.GOLD, c["name"] + ".dot.gz"))
     r = subprocess.run([os.path.join(BIN, "abyss-bloom-dbg"), "-k21", "-K5", "-b64k", "-g", dot, fq], capture_output=True, text=True)
     assert r.returncode != 0 and "spaced seed" in r.stderr
 

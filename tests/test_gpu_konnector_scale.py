@@ -4,24 +4,14 @@ in one batch and in four."""
 import hashlib
 import json
 import os
-import subprocess
 
 import pytest
 
+import parity
 from abyss_b200.synth import ReadSet
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EXE = os.path.join(ROOT, "abyss_b200", "lib", "abyss-bloom")
-CASES = json.load(open(os.path.join(ROOT, "tests", "golden", "konnector_scale.json")))
-
-
-def sha256_file(path):
-    h = hashlib.sha256()
-    with open(path, "rb") as f:
-        for blk in iter(lambda: f.read(1 << 22), b""):
-            h.update(blk)
-    return h.hexdigest()
+CASES = json.load(open(os.path.join(parity.GOLD, "konnector_scale.json")))
 
 
 @pytest.fixture(scope="module")
@@ -41,8 +31,8 @@ def test_konnector_scale(abb, reads, case, batch):
     d, fqs = reads
     out = str(d / "o.bloom")
     extra = [f"--batch-reads={batch}"] if batch else []
-    r = subprocess.run([EXE, "build", *case["args"], *extra, out, fqs[case["name"]]], capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    assert r.stderr == case["stderr"]
-    assert sha256_file(out) == case["sha256"]
+    r = parity.run(os.path.join(parity.BIN, "abyss-bloom"), "build", *case["args"], *extra, out, fqs[case["name"]])
+    assert r.stderr.decode() == case["stderr"]
+    with open(out, "rb") as f:
+        assert hashlib.file_digest(f, "sha256").hexdigest() == case["sha256"]
     os.remove(out)

@@ -3,144 +3,64 @@
 through the C ABI in one batch and in batches of 997 reads, with and without tiles, and through abyss-bloom-dbg (FASTA, read
 log, -T trace, counters); the -g dump and the -C/-R coverage track; `abyss-bloom graph` and `abyss-bloom trim`; and the masked
 K1 hashes against the C oracle."""
-import gzip
-import hashlib
 import json
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 
+import parity
+from make_golden_kwidth import GRAPH_FILTERS, TRIM_FILTERS, write_graph_inputs, write_trim_inputs
+
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GOLD = os.path.join(ROOT, "tests", "golden")
-BIN = os.path.join(ROOT, "abyss_b200", "lib")
-sys.path.insert(0, GOLD)
-from make_golden_kwidth import (GRAPH_FILTERS, TRIM_FILTERS, blank_trace, raw_reads, reader_view, write_fastq,  # noqa: E402
-                                write_graph_inputs, write_trim_inputs)
-
-CASES = json.load(open(os.path.join(GOLD, "kwidth_cases.json")))
+CASES = json.load(open(os.path.join(parity.GOLD, "kwidth_cases.json")))
 ASM = CASES["assembler"]
-
-
-def md5(data):
-    return hashlib.md5(data).hexdigest()
-
-
-def sha256(data):
-    return hashlib.sha256(data).hexdigest()
-
-
-def _read_log(ids, codes):
-    from abyss_b200.capi import READ_CODES
-    return "read_id\tresult\n" + "".join(f"{i}\t{READ_CODES[c]}\n" for i, c in zip(ids, codes))
 
 
 @pytest.mark.parametrize("case", ASM, ids=[c["name"] for c in ASM])
 def test_assembler_c_abi(abb, monkeypatch, case):
-    from abyss_b200.capi import Filter, bloom_dbg
-    ids, seqs = map(list, zip(*reader_view(raw_reads(case["reads"]))))
-    mask = case.get("mask", "")
-    if "counters_sha256" in case:
-        f = Filter.counting(case["counters"], case["H"], case["k"], case["kc"])
-        f.insert_reads(seqs)
-        assert sha256(f.download().tobytes()) == case["counters_sha256"]
-        f.close()
-    for batch in (None, 997):
-        fasta, codes = bloom_dbg(ids, seqs, case["k"], case["kc"], case["H"], counters=case["counters"], batch_reads=batch,
-                                 read_log=True, mask=mask)
-        assert fasta.count(">") == case["n_contigs"], batch
-        assert md5(fasta.encode()) == case["fasta_md5"], batch
-        assert md5(_read_log(ids, codes).encode()) == case["readlog_md5"], batch
-    monkeypatch.setenv("ABB_NO_TILES", "1")
-    fasta, _ = bloom_dbg(ids, seqs, case["k"], case["kc"], case["H"], counters=case["counters"], mask=mask)
-    assert md5(fasta.encode()) == case["fasta_md5"], "ABB_NO_TILES=1"
+    parity.check_assembler_c_abi(case, monkeypatch)
 
 
 @pytest.mark.parametrize("case", ASM, ids=[c["name"] for c in ASM])
 def test_assembler_cli(abb, tmp_path, case):
-    fq, fa, log, tr, bf = (str(tmp_path / x) for x in ("reads.fq", "out.fa", "read.log", "trace.tsv", "c.bloom"))
-    write_fastq(raw_reads(case["reads"]), fq)
-    opt = [case["opt"]] if case["opt"] else []
-    r = subprocess.run([os.path.join(BIN, "abyss-bloom-dbg"), f"-k{case['k']}", *opt, f"--kc={case['kc']}", f"-b{case['b']}",
-                        f"-H{case['H']}", "-j1", f"--read-log={log}", "-T", tr, "-o", fa, fq], capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    assert md5(open(fa, "rb").read()) == case["fasta_md5"]
-    assert md5(open(log, "rb").read()) == case["readlog_md5"]
-    assert sha256(blank_trace(open(tr).read()).encode()) == case["trace_sha256"]
-    if "counters_sha256" in case:
-        r = subprocess.run([os.path.join(BIN, "abyss-bloom"), "build", "-k", str(case["k"]), "-t", "counting", f"-b{case['counters']}",
-                            f"-H{case['H']}", bf, fq], capture_output=True, text=True)
-        assert r.returncode == 0, r.stderr
-        blob = open(bf, "rb").read()
-        assert sha256(blob[blob.index(b"[HeaderEnd]\n") + 12:]) == case["counters_sha256"]
+    parity.check_assembler_cli(case, tmp_path)
 
 
 @pytest.mark.parametrize("case", CASES["dbg_graph"], ids=[c["name"] for c in CASES["dbg_graph"]])
 def test_graphviz_dump(abb, tmp_path, case):
-    fq, dot = str(tmp_path / "reads.fq"), str(tmp_path / "g.dot")
-    write_fastq(raw_reads(case["reads"]), fq)
-    r = subprocess.run([os.path.join(BIN, "abyss-bloom-dbg"), f"-k{case['k']}", f"--kc={case['kc']}", f"-b{case['b']}", f"-H{case['H']}",
-                        "-g", dot, "--batch-reads=700", "-o", os.devnull, fq], capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    data = open(dot, "rb").read()
-    assert (len(data), data.count(b"\n")) == (case["bytes"], case["lines"])
-    assert sha256(data) == case["sha256"]
+    parity.check_dbg_graph(case, tmp_path)
 
 
 @pytest.mark.parametrize("case", CASES["covtrack"], ids=[c["name"] for c in CASES["covtrack"]])
 def test_coverage_track(abb, tmp_path, case):
-    from abyss_b200.synth import ReadSet
-    from make_golden_covtrack import ref_fasta
-    fq, ref, wig = str(tmp_path / "reads.fq"), str(tmp_path / "ref.fa"), str(tmp_path / "cov.wig")
-    s = case["reads"]
-    write_fastq(raw_reads(s), fq)
-    ref_fasta(ReadSet.from_coverage(s["seed"], s["genome"], s["cov"], s["L"], s["err"]), ref)
-    r = subprocess.run([os.path.join(BIN, "abyss-bloom-dbg"), f"-k{case['k']}", f"--kc={case['kc']}", f"-b{case['b']}", f"-H{case['H']}",
-                        "-C", wig, "-R", ref, "-o", os.devnull, fq], capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    data = open(wig, "rb").read()
-    assert (len(data), data.count(b"\n")) == (case["bytes"], case["lines"])
-    assert sha256(data) == case["sha256"]
+    parity.check_coverage_track(case, tmp_path)
 
 
 @pytest.fixture(scope="module")
 def graph_work(tmp_path_factory, abb):
     d = str(tmp_path_factory.mktemp("kwg"))
     write_graph_inputs(d)
-    for f in GRAPH_FILTERS.values():
-        r = subprocess.run([os.path.join(BIN, "abyss-bloom"), *f["args"]], cwd=d, capture_output=True)
-        assert r.returncode == 0, r.stderr.decode()
+    parity.build_filters(GRAPH_FILTERS.values(), d)
     return d
 
 
 @pytest.mark.parametrize("case", CASES["graph"], ids=[c["name"] for c in CASES["graph"]])
 def test_bloom_graph_cli(graph_work, case):
-    r = subprocess.run([os.path.join(BIN, "abyss-bloom"), *case["args"]], cwd=graph_work, capture_output=True)
-    assert r.returncode == case["rc"], r.stderr.decode()
-    assert r.stderr.decode() == case["stderr"]
-    assert (len(r.stdout), r.stdout.count(b"\n")) == (case["bytes"], case["lines"])
-    assert r.stdout == gzip.open(os.path.join(GOLD, f"kwidth_{case['name']}.dot.gz"), "rb").read()
+    parity.check_bloom_graph_cli(case, graph_work, os.path.join(parity.GOLD, f"kwidth_{case['name']}.dot.gz"))
 
 
 @pytest.fixture(scope="module")
 def trim_work(tmp_path_factory, abb):
     d = str(tmp_path_factory.mktemp("kwt"))
     write_trim_inputs(d)
-    for f in TRIM_FILTERS:
-        r = subprocess.run([os.path.join(BIN, "abyss-bloom"), *f["args"]], cwd=d, capture_output=True)
-        assert r.returncode == 0, r.stderr.decode()
+    parity.build_filters(TRIM_FILTERS, d)
     return d
 
 
 @pytest.mark.parametrize("case", CASES["trim"], ids=[c["name"] for c in CASES["trim"]])
 def test_trim_cli(trim_work, case):
-    r = subprocess.run([os.path.join(BIN, "abyss-bloom"), *case["args"]], cwd=trim_work, capture_output=True)
-    assert r.returncode == case["rc"], r.stderr.decode()
-    assert r.stderr.decode() == case["stderr"]
-    assert md5(r.stdout) == case["stdout_md5"]
+    parity.check_trim_cli(case, trim_work)
 
 
 def _masks(k):

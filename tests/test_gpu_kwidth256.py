@@ -3,26 +3,21 @@ unmodified reference built with MAX_KMER = 256 (tests/golden/kwidth256_cases.jso
 assembler through the C ABI in one batch and in batches of 997 reads, with and without tiles, and through abyss-bloom-dbg; the
 -g dump and the -C/-R coverage track; `abyss-bloom graph`, Konnector filters and `trim`; AdjList in every output format; the
 K1 hashes against the C oracle; and k = 257 refused."""
-import gzip
-import hashlib
 import json
 import os
 import subprocess
-import sys
 
 import numpy as np
 import pytest
 
-pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GOLD = os.path.join(ROOT, "tests", "golden")
-BIN = os.path.join(ROOT, "abyss_b200", "lib")
-sys.path.insert(0, GOLD)
-from make_golden_kwidth import blank_trace, raw_reads, reader_view, write_fastq, write_graph_inputs, write_trim_inputs  # noqa: E402
-from make_golden_kwidth256 import GRAPH_FILTERS, adjlist_input  # noqa: E402
-import overlap_cases as oc  # noqa: E402
+import overlap_cases as oc
+import parity
+from make_golden_kwidth import write_fastq, write_graph_inputs, write_trim_inputs
+from make_golden_kwidth256 import GRAPH_FILTERS, adjlist_input
 
-CASES = json.load(open(os.path.join(GOLD, "kwidth256_cases.json")))
+pytestmark = pytest.mark.gpu
+BIN = parity.BIN
+CASES = json.load(open(os.path.join(parity.GOLD, "kwidth256_cases.json")))
 ASM = CASES["assembler"]
 ENV = dict(os.environ, ABYSS_MAX_KMER="256")  # the command-line programs' MAX_KMER (192 without it)
 
@@ -35,104 +30,37 @@ def max_kmer_256(abb):
     abb.set_max_kmer(192)
 
 
-def md5(data):
-    return hashlib.md5(data).hexdigest()
-
-
-def sha256(data):
-    return hashlib.sha256(data).hexdigest()
-
-
-def _read_log(ids, codes):
-    from abyss_b200.capi import READ_CODES
-    return "read_id\tresult\n" + "".join(f"{i}\t{READ_CODES[c]}\n" for i, c in zip(ids, codes))
-
-
 @pytest.mark.parametrize("case", ASM, ids=[c["name"] for c in ASM])
 def test_assembler_c_abi(abb, monkeypatch, case):
-    from abyss_b200.capi import Filter, bloom_dbg
-    ids, seqs = map(list, zip(*reader_view(raw_reads(case["reads"]))))
-    mask = case.get("mask", "")
-    if "counters_sha256" in case:
-        f = Filter.counting(case["counters"], case["H"], case["k"], case["kc"])
-        f.insert_reads(seqs)
-        assert sha256(f.download().tobytes()) == case["counters_sha256"]
-        f.close()
-    for batch in (None, 997):
-        fasta, codes = bloom_dbg(ids, seqs, case["k"], case["kc"], case["H"], counters=case["counters"], batch_reads=batch,
-                                 read_log=True, mask=mask)
-        assert fasta.count(">") == case["n_contigs"], batch
-        assert md5(fasta.encode()) == case["fasta_md5"], batch
-        assert md5(_read_log(ids, codes).encode()) == case["readlog_md5"], batch
-    monkeypatch.setenv("ABB_NO_TILES", "1")
-    fasta, _ = bloom_dbg(ids, seqs, case["k"], case["kc"], case["H"], counters=case["counters"], mask=mask)
-    assert md5(fasta.encode()) == case["fasta_md5"], "ABB_NO_TILES=1"
+    parity.check_assembler_c_abi(case, monkeypatch)
 
 
 @pytest.mark.parametrize("case", ASM, ids=[c["name"] for c in ASM])
 def test_assembler_cli(abb, tmp_path, case):
-    fq, fa, log, tr, bf = (str(tmp_path / x) for x in ("reads.fq", "out.fa", "read.log", "trace.tsv", "c.bloom"))
-    write_fastq(raw_reads(case["reads"]), fq)
-    opt = [case["opt"]] if case["opt"] else []
-    r = subprocess.run([os.path.join(BIN, "abyss-bloom-dbg"), f"-k{case['k']}", *opt, f"--kc={case['kc']}", f"-b{case['b']}",
-                        f"-H{case['H']}", "-j1", f"--read-log={log}", "-T", tr, "-o", fa, fq], capture_output=True, env=ENV, text=True)
-    assert r.returncode == 0, r.stderr
-    assert md5(open(fa, "rb").read()) == case["fasta_md5"]
-    assert md5(open(log, "rb").read()) == case["readlog_md5"]
-    assert sha256(blank_trace(open(tr).read()).encode()) == case["trace_sha256"]
-    if "counters_sha256" in case:
-        r = subprocess.run([os.path.join(BIN, "abyss-bloom"), "build", "-k", str(case["k"]), "-t", "counting", f"-b{case['counters']}",
-                            f"-H{case['H']}", bf, fq], capture_output=True, env=ENV, text=True)
-        assert r.returncode == 0, r.stderr
-        blob = open(bf, "rb").read()
-        assert sha256(blob[blob.index(b"[HeaderEnd]\n") + 12:]) == case["counters_sha256"]
+    parity.check_assembler_cli(case, tmp_path, env=ENV)
 
 
 @pytest.mark.parametrize("case", CASES["dbg_graph"], ids=[c["name"] for c in CASES["dbg_graph"]])
 def test_graphviz_dump(abb, tmp_path, case):
-    fq, dot = str(tmp_path / "reads.fq"), str(tmp_path / "g.dot")
-    write_fastq(raw_reads(case["reads"]), fq)
-    r = subprocess.run([os.path.join(BIN, "abyss-bloom-dbg"), f"-k{case['k']}", f"--kc={case['kc']}", f"-b{case['b']}", f"-H{case['H']}",
-                        "-g", dot, "--batch-reads=700", "-o", os.devnull, fq], capture_output=True, env=ENV, text=True)
-    assert r.returncode == 0, r.stderr
-    data = open(dot, "rb").read()
-    assert (len(data), data.count(b"\n")) == (case["bytes"], case["lines"])
-    assert sha256(data) == case["sha256"]
+    parity.check_dbg_graph(case, tmp_path, ENV)
 
 
 @pytest.mark.parametrize("case", CASES["covtrack"], ids=[c["name"] for c in CASES["covtrack"]])
 def test_coverage_track(abb, tmp_path, case):
-    from abyss_b200.synth import ReadSet
-    from make_golden_covtrack import ref_fasta
-    fq, ref, wig = str(tmp_path / "reads.fq"), str(tmp_path / "ref.fa"), str(tmp_path / "cov.wig")
-    s = case["reads"]
-    write_fastq(raw_reads(s), fq)
-    ref_fasta(ReadSet.from_coverage(s["seed"], s["genome"], s["cov"], s["L"], s["err"]), ref)
-    r = subprocess.run([os.path.join(BIN, "abyss-bloom-dbg"), f"-k{case['k']}", f"--kc={case['kc']}", f"-b{case['b']}", f"-H{case['H']}",
-                        "-C", wig, "-R", ref, "-o", os.devnull, fq], capture_output=True, env=ENV, text=True)
-    assert r.returncode == 0, r.stderr
-    data = open(wig, "rb").read()
-    assert (len(data), data.count(b"\n")) == (case["bytes"], case["lines"])
-    assert sha256(data) == case["sha256"]
+    parity.check_coverage_track(case, tmp_path, ENV)
 
 
 @pytest.fixture(scope="module")
 def graph_work(tmp_path_factory, abb):
     d = str(tmp_path_factory.mktemp("kwg256"))
     write_graph_inputs(d)
-    for f in GRAPH_FILTERS.values():
-        r = subprocess.run([os.path.join(BIN, "abyss-bloom"), *f["args"]], cwd=d, capture_output=True, env=ENV)
-        assert r.returncode == 0, r.stderr.decode()
+    parity.build_filters(GRAPH_FILTERS.values(), d, ENV)
     return d
 
 
 @pytest.mark.parametrize("case", CASES["graph"], ids=[c["name"] for c in CASES["graph"]])
 def test_bloom_graph_cli(graph_work, case):
-    r = subprocess.run([os.path.join(BIN, "abyss-bloom"), *case["args"]], cwd=graph_work, capture_output=True, env=ENV)
-    assert r.returncode == case["rc"], r.stderr.decode()
-    assert r.stderr.decode() == case["stderr"]
-    assert (len(r.stdout), r.stdout.count(b"\n")) == (case["bytes"], case["lines"])
-    assert r.stdout == gzip.open(os.path.join(GOLD, f"kwidth256_{case['name']}.dot.gz"), "rb").read()
+    parity.check_bloom_graph_cli(case, graph_work, os.path.join(parity.GOLD, f"kwidth256_{case['name']}.dot.gz"), ENV)
 
 
 @pytest.fixture(scope="module")
@@ -142,10 +70,10 @@ def konnector_work(tmp_path_factory, abb):
     write_trim_inputs(d)
     out = {}
     for c in CASES["konnector"]:
-        r = subprocess.run([os.path.join(BIN, "abyss-bloom"), *c["args"]], cwd=d, capture_output=True, env=ENV)
-        rec = {"rc": r.returncode, "stdout_md5": md5(r.stdout), "stderr": r.stderr.decode()}
+        r = parity.abyss_bloom(*c["args"], cwd=d, env=ENV)
+        rec = {"rc": r.returncode, "stdout_md5": parity.md5(r.stdout), "stderr": r.stderr.decode()}
         if "file" in c and os.path.exists(os.path.join(d, c["file"])):
-            rec["sha256"] = sha256(open(os.path.join(d, c["file"]), "rb").read())
+            rec["sha256"] = parity.sha256(open(os.path.join(d, c["file"]), "rb").read())
         out[c["name"]] = rec
     return d, out
 
@@ -162,10 +90,7 @@ def test_konnector_cli(konnector_work, case):
 
 @pytest.mark.parametrize("case", CASES["trim"], ids=[c["name"] for c in CASES["trim"]])
 def test_trim_cli(konnector_work, case):
-    r = subprocess.run([os.path.join(BIN, "abyss-bloom"), *case["args"]], cwd=konnector_work[0], capture_output=True, env=ENV)
-    assert r.returncode == case["rc"], r.stderr.decode()
-    assert r.stderr.decode() == case["stderr"]
-    assert md5(r.stdout) == case["stdout_md5"]
+    parity.check_trim_cli(case, konnector_work[0], ENV)
 
 
 @pytest.mark.parametrize("case", CASES["adjlist"], ids=[c["name"] for c in CASES["adjlist"]])
@@ -176,7 +101,7 @@ def test_adjlist_cli(abb, tmp_path, case):
     r = subprocess.run([exe] + oc.command_args(t, fa), capture_output=True, env=ENV)
     assert r.returncode == 0, r.stderr.decode()
     got = oc.normalise(r.stdout, exe).replace(fa.encode(), b"IN.fa")
-    assert (len(got), sha256(got)) == (case["bytes"], case["sha256"])
+    assert (len(got), parity.sha256(got)) == (case["bytes"], case["sha256"])
 
 
 def _reads(k):

@@ -4,9 +4,9 @@ reference, tests/golden/make_golden.py), and the per-read outcome log must match
 import json
 import os
 
-import numpy as np
 import pytest
 
+import parity
 from abyss_b200.synth import ReadSet
 
 pytestmark = pytest.mark.gpu
@@ -22,7 +22,7 @@ def load_case(golden_dir, name):
 @pytest.mark.parametrize("name", ["e2e_g20k_k32", "e2e_g30k_k64", "e2e_g10k_k25_small"])
 @pytest.mark.parametrize("batch", [None, 997])
 def test_fasta_identical_to_reference(abb, golden_dir, name, batch):
-    from abyss_b200.capi import fixed_length_reads, bloom_dbg, READ_CODES
+    from abyss_b200.capi import fixed_length_reads, bloom_dbg
     c, rs = load_case(golden_dir, name)
     ids = [rs.read_id(i) for i in range(rs.n)]
     fasta, codes = bloom_dbg(ids, fixed_length_reads(rs.ascii(0, rs.n)), c["k"], c["kc"], c["H"], counters=c["counters"],
@@ -30,10 +30,7 @@ def test_fasta_identical_to_reference(abb, golden_dir, name, batch):
     want = open(os.path.join(golden_dir, name + ".fa")).read()
     assert fasta.count(">") == c["n_contigs"]
     assert fasta == want
-    # --read-log parity
-    log = open(os.path.join(golden_dir, name + ".readlog.tsv")).read().split("\n")[1:-1]
-    got = [f"{ids[i]}\t{READ_CODES[codes[i]]}" for i in range(rs.n)]
-    assert got == log
+    assert parity.read_log(ids, codes) == open(os.path.join(golden_dir, name + ".readlog.tsv")).read()
 
 
 def test_mixed_reads_edge_cases(abb, golden_dir):
@@ -80,7 +77,7 @@ MASK_CASES = json.load(open(os.path.join(os.path.dirname(__file__), "golden", "m
 def test_spaced_seeds_identical_to_reference(abb, golden_dir, case):
     # -K / --qr-seed / -s: the spaced seed changes the hash (pass 1 and every Bloom probe), vertex identity
     # (RollingBloomDBGVertex::compare orients by the full k-mer) and pathToSeq ('N' where no vertex writes a column)
-    from abyss_b200.capi import bloom_dbg, fixed_length_reads, kmer_pair_seed, qr_seed_pair, READ_CODES
+    from abyss_b200.capi import bloom_dbg, fixed_length_reads, kmer_pair_seed, qr_seed_pair
     if case["opt"].startswith("-K"):
         assert kmer_pair_seed(case["k"], int(case["opt"][2:])) == case["mask"]
     else:
@@ -97,8 +94,7 @@ def test_spaced_seeds_identical_to_reference(abb, golden_dir, case):
     assert fasta.count(">") == case["n_contigs"]
     assert fasta == want
     if case.get("readlog"):
-        log = open(os.path.join(golden_dir, case["name"] + ".readlog.tsv")).read().split("\n")[1:-1]
-        assert [f"{ids[i]}\t{READ_CODES[codes[i]]}" for i in range(len(ids))] == log
+        assert parity.read_log(ids, codes) == open(os.path.join(golden_dir, case["name"] + ".readlog.tsv")).read()
 
 
 def test_spaced_seed_validation(abb):
@@ -125,6 +121,7 @@ def test_assembler_reset_reuses_handle(abb, golden_dir):
     # abb_assembler_reset: a second assembly on the same handles gives the same bytes
     from abyss_b200.capi import fixed_length_reads, Filter, Assembler
     c, rs = load_case(golden_dir, "e2e_g20k_k32")
+    ids = [rs.read_id(i) for i in range(rs.n)]
     reads = fixed_length_reads(rs.ascii(0, rs.n))
     f = Filter.counting(c["counters"], c["H"], c["k"], c["kc"])
     a = Assembler(f)
@@ -133,7 +130,7 @@ def test_assembler_reset_reuses_handle(abb, golden_dir):
         f.clear()
         a.reset()
         f.insert_reads(reads)
-        outs.append("".join(f">{i} {len(s)} {cv} read:{rs.read_id(r)}\n{s}\n" for i, (r, s, cv) in enumerate(a.process_reads(reads))))
+        outs.append(a.assemble(ids, reads)[0])
     a.close()
     f.close()
     assert outs[0] == outs[1] == open(os.path.join(golden_dir, "e2e_g20k_k32.fa")).read()
@@ -147,29 +144,19 @@ def test_hash_counts_identical_to_reference(abb, golden_dir, tmp_path, case):
     # H = 1, 2, 5, 8, 9: the MAXH = 4 kernels with lanes that have nothing to probe, and the MAXH = 8 and 32 kernels.  Counters,
     # FASTA and read log against the reference's -j1 run (tests/golden/make_golden_hashnum.py), through the C ABI as one batch
     # and in batches of 997 reads, and through abyss-bloom-dbg
-    import hashlib
-    import subprocess
-    from abyss_b200.capi import fixed_length_reads, bloom_dbg, READ_CODES, Filter
+    from abyss_b200.capi import fixed_length_reads, bloom_dbg, Filter
     c, rs = load_case(golden_dir, case["reads"])
     H = case["H"]
     ids = [rs.read_id(i) for i in range(rs.n)]
     reads = fixed_length_reads(rs.ascii(0, rs.n))
     f = Filter.counting(c["counters"], H, c["k"], c["kc"])
     f.insert_reads(reads)
-    assert hashlib.sha256(f.download().tobytes()).hexdigest() == case["counters_sha256"]
+    assert parity.sha256(f.download().tobytes()) == case["counters_sha256"]
     f.close()
-    md5 = lambda b: hashlib.md5(b).hexdigest()  # noqa: E731
     for batch in (None, 997):
         fasta, codes = bloom_dbg(ids, reads, c["k"], c["kc"], H, counters=c["counters"], batch_reads=batch, read_log=True)
-        log = "read_id\tresult\n" + "".join(f"{ids[i]}\t{READ_CODES[codes[i]]}\n" for i in range(rs.n))
-        assert fasta.count(">") == case["n_contigs"], batch
-        assert md5(fasta.encode()) == case["fasta_md5"], batch
-        assert md5(log.encode()) == case["readlog_md5"], batch
-    fq, fa, log = (str(tmp_path / x) for x in ("reads.fq", "out.fa", "readlog.tsv"))
+        parity.check_unitigs(case, fasta, parity.read_log(ids, codes))
+    fq = str(tmp_path / "reads.fq")
     rs.write_fastq(fq)
-    exe = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "abyss_b200", "lib", "abyss-bloom-dbg")
-    r = subprocess.run([exe, f"-k{c['k']}", f"--kc={c['kc']}", f"-b{c['b']}", f"-H{H}", "-j1", f"--read-log={log}", "-o", fa, fq],
-                       capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    assert md5(open(fa, "rb").read()) == case["fasta_md5"]
-    assert md5(open(log, "rb").read()) == case["readlog_md5"]
+    fasta, log, _ = parity.bloom_dbg_cli(dict(c, H=H), fq, tmp_path)
+    parity.check_unitigs(case, fasta, log)

@@ -1,21 +1,14 @@
 """CPU: the arithmetic helpers shared by host and device code (exact modulo, split rotations, ntHash
 rolls, 2-bit k-mers) against the oracle, and the CLI's FASTA/FASTQ reader semantics
 (DataLayer/FastaReader.cpp:130-421: Casava chastity filter, masked-end trimming, case folding, quality trim)."""
-import os
 import subprocess
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+import parity
+
+host_arith = parity.harness("host_arith", "tests/host_arith/host_arith.cpp", parity.ORACLE)
 
 
-def build(tmp_path):
-    exe = str(tmp_path / "host_arith")
-    subprocess.run(["g++", "-std=c++17", "-O2", "-pthread", "-Wno-unknown-pragmas", "-o", exe, os.path.join(ROOT, "tests", "host_arith", "host_arith.cpp"),
-                    os.path.join(ROOT, "oracle", "abyss_oracle.c")], check=True, capture_output=True)
-    return exe
-
-
-def test_host_arith_and_reader(tmp_path):
-    exe = build(tmp_path)
+def test_host_arith_and_reader(host_arith, tmp_path):
     fq = tmp_path / "in.fq"
     fq.write_text(
         "# a comment line\n"
@@ -24,7 +17,7 @@ def test_host_arith_and_reader(tmp_path):
         "@r3/1\nACGTacgtAC\n+\n##IIIIII##\n"                            # quality trim at q>=3 removes '#' (q=2) ends
         ">f1 some comment\nACGT\nACGT\nAC\n"                            # multi-line FASTA
         ">f2\nacgt\n")                                                  # all masked -> empty read
-    r = subprocess.run([exe, str(fq), "3"], capture_output=True, text=True)
+    r = subprocess.run([host_arith, str(fq), "3"], capture_output=True, text=True)
     assert r.returncode == 0, r.stdout + r.stderr
     lines = r.stdout.strip().split("\n")
     assert lines[-1] == "HOST_ARITH_OK"

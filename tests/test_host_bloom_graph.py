@@ -2,21 +2,16 @@
 kernel runs (kmer_hash_part, nbr_lane, nbr_mask of abyss_b200/csrc/abb_graph.cuh), driven by the single-thread harness
 tests/host_bloom_graph on filters the C oracle rebuilds -- writes the bytes of the unmodified reference's dump on every case of
 tests/golden/bloom_graph_cases.json (tests/golden/make_golden_bloom_graph.py) that prints one."""
-import gzip
-import hashlib
 import json
 import os
-import subprocess
-import sys
 
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GOLD = os.path.join(ROOT, "tests", "golden")
-sys.path.insert(0, GOLD)
-from make_golden_bloom_graph import RECIPES, write_inputs  # noqa: E402
+import parity
+from make_golden_bloom_graph import RECIPES, write_inputs
 
-CASES = [c for c in json.load(open(os.path.join(GOLD, "bloom_graph_cases.json"))) if c["harness"]]
+CASES = [c for c in json.load(open(os.path.join(parity.GOLD, "bloom_graph_cases.json"))) if c["harness"]]
+host_bloom_graph = parity.harness("host_bloom_graph", "tests/host_bloom_graph/host_bloom_graph.cpp", parity.ORACLE)
 
 
 def harness_args(args):
@@ -48,25 +43,15 @@ def harness_args(args):
 
 @pytest.fixture(scope="module")
 def work(tmp_path_factory):
-    d = tmp_path_factory.mktemp("bg")
-    exe = str(d / "host_bloom_graph")
-    subprocess.run(["g++", "-std=c++17", "-O2", "-Wno-unknown-pragmas", "-pthread", "-o", exe,
-                    os.path.join(ROOT, "tests", "host_bloom_graph", "host_bloom_graph.cpp"), os.path.join(ROOT, "oracle", "abyss_oracle.c")],
-                   check=True, capture_output=True)
-    write_inputs(str(d), large=any(c["name"] == "large" for c in CASES))
-    return str(d), exe
+    d = str(tmp_path_factory.mktemp("bg"))
+    write_inputs(d, large=any(c["name"] == "large" for c in CASES))
+    return d
 
 
 @pytest.mark.parametrize("case", CASES, ids=[c["name"] for c in CASES])
-def test_bloom_graph_dump(work, case):
-    d, exe = work
-    r = subprocess.run([exe, *harness_args(case["args"])], cwd=d, capture_output=True)
-    assert r.returncode == 0, r.stderr.decode()
-    assert (len(r.stdout), r.stdout.count(b"\n")) == (case["bytes"], case["lines"])
-    full = os.path.join(GOLD, f"bloom_graph_{case['name']}.dot.gz")
-    if os.path.exists(full):
-        assert r.stdout == gzip.open(full, "rb").read()
-    assert hashlib.sha256(r.stdout).hexdigest() == case["sha256"]
+def test_bloom_graph_dump(host_bloom_graph, work, case):
+    r = parity.run(host_bloom_graph, *harness_args(case["args"]), cwd=work)
+    parity.check_dump(r.stdout, case, os.path.join(parity.GOLD, f"bloom_graph_{case['name']}.dot.gz"))
 
 
 def test_harness_args():

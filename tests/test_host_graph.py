@@ -1,30 +1,16 @@
 """CPU: the GraphViz dump `abyss-bloom-dbg -g` -- the product's traversal (abyss_b200/host/graph_dump.h) and the out-edge walk
 the CUDA kernel runs (successors_chain, abyss_b200/csrc/abb_graph.cuh), driven by the single-thread harness tests/host_graph
 on an oracle-built filter -- writes the bytes of the unmodified reference's -g file (tests/golden/make_golden_graph.py)."""
-import gzip
-import hashlib
 import json
 import os
-import subprocess
 
 import pytest
 
-import sys
+import parity
+from make_golden_graph import write_reads
 
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden"))
-from make_golden_graph import write_reads  # noqa: E402
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GOLD = os.path.join(ROOT, "tests", "golden")
-CASES = json.load(open(os.path.join(GOLD, "graph_cases.json")))
-
-
-@pytest.fixture(scope="module")
-def harness(tmp_path_factory):
-    exe = str(tmp_path_factory.mktemp("hg") / "host_graph")
-    subprocess.run(["g++", "-std=c++17", "-O2", "-Wno-unknown-pragmas", "-pthread", "-o", exe, os.path.join(ROOT, "tests", "host_graph", "host_graph.cpp"),
-                    os.path.join(ROOT, "oracle", "abyss_oracle.c")], check=True, capture_output=True)
-    return exe
+CASES = json.load(open(os.path.join(parity.GOLD, "graph_cases.json")))
+harness = parity.harness("host_graph", "tests/host_graph/host_graph.cpp", parity.ORACLE)
 
 
 @pytest.mark.parametrize("case", CASES, ids=[c["name"] for c in CASES])
@@ -32,10 +18,5 @@ def test_graph_dump(harness, tmp_path, case):
     c = case
     fq = str(tmp_path / "r.fq")
     write_reads(c, fq)
-    r = subprocess.run([harness, str(c["k"]), str(c["kc"]), str(c["H"]), str(c["counters"]), fq], capture_output=True)
-    assert r.returncode == 0, r.stderr.decode()
-    assert len(r.stdout) == c["bytes"] and r.stdout.count(b"\n") == c["lines"]
-    assert hashlib.sha256(r.stdout).hexdigest() == c["sha256"]
-    full = os.path.join(GOLD, c["name"] + ".dot.gz")
-    if os.path.exists(full):
-        assert r.stdout == gzip.open(full, "rb").read()
+    r = parity.run(harness, c["k"], c["kc"], c["H"], c["counters"], fq)
+    parity.check_dump(r.stdout, c, os.path.join(parity.GOLD, c["name"] + ".dot.gz"))

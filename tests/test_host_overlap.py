@@ -3,7 +3,6 @@ call) and the product's AdjList command line and graph writers (abyss_b200/host/
 single-thread harness tests/host_overlap, against the unmodified reference AdjList: committed goldens
 (tests/golden/make_golden_overlap.py, tests/golden/make_golden_ref_live.py)."""
 import gzip
-import hashlib
 import json
 import os
 import subprocess
@@ -11,18 +10,11 @@ import subprocess
 import pytest
 
 import overlap_cases as oc
+import parity
 import ref_golden
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GOLD = os.path.join(ROOT, "tests", "golden")
-
-
-@pytest.fixture(scope="module")
-def harness(tmp_path_factory):
-    exe = str(tmp_path_factory.mktemp("ho") / "AdjList")
-    subprocess.run(["g++", "-std=c++17", "-O2", "-Wno-unknown-pragmas", "-o", exe, os.path.join(ROOT, "tests", "host_overlap", "host_overlap.cpp")],
-                   check=True, capture_output=True)
-    return exe
+GOLD = parity.GOLD
+harness = parity.harness("AdjList", "tests/host_overlap/host_overlap.cpp")
 
 
 def run_case(exe, case, tmp_path):
@@ -40,7 +32,7 @@ def test_goldens(harness, tmp_path):
     for c in cases:
         got = run_case(harness, c, tmp_path)
         assert len(got) == want[c["name"]]["bytes"], c["name"]
-        assert hashlib.sha256(got).hexdigest() == want[c["name"]]["sha256"], c["name"]
+        assert parity.sha256(got) == want[c["name"]]["sha256"], c["name"]
         full = os.path.join(GOLD, "overlap_" + c["name"] + ".txt")
         if os.path.exists(full):
             assert got == open(full, "rb").read()

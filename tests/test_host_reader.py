@@ -10,17 +10,10 @@ import subprocess
 
 import pytest
 
+import parity
 import ref_golden
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-@pytest.fixture(scope="module")
-def exe(tmp_path_factory):
-    out = str(tmp_path_factory.mktemp("rd") / "host_reader")
-    subprocess.run(["g++", "-std=c++17", "-O2", "-pthread", "-Wall", "-o", out, os.path.join(ROOT, "tests", "host_reader", "host_reader.cpp")],
-                   check=True, capture_output=True)
-    return out
+exe = parity.harness("host_reader", "tests/host_reader/host_reader.cpp", flag="-Wall")
 
 
 def run(exe, *args, env=None):

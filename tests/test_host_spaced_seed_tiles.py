@@ -7,40 +7,25 @@ would splice the wrong continuation.  Dropping a seeded subset of the tiles, as 
 The 1 M-read case sp_m1_k80_K32 takes the single-lane harness minutes; it runs on the GPU only
 (tests/test_gpu_spaced_seed_tiles.py)."""
 import gzip
-import hashlib
 import json
 import os
 import re
-import subprocess
-import sys
 
 import pytest
 
+import parity  # first: it puts tests/golden on the path
+import make_golden_kwidth as kwidth
+import make_golden_spaced_tiles as spaced
 from abyss_b200.synth import ReadSet
+from parity import md5
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GOLD = os.path.join(ROOT, "tests", "golden")
-sys.path.insert(0, GOLD)
-import make_golden_kwidth as kwidth  # noqa: E402
-import make_golden_spaced_tiles as spaced  # noqa: E402
+GOLD = parity.GOLD
 
 MASK = json.load(open(os.path.join(GOLD, "mask_cases.json")))
 KWIDTH = [c for c in json.load(open(os.path.join(GOLD, "kwidth_cases.json")))["assembler"] if c["opt"]]
 SPACED = [c for c in json.load(open(os.path.join(GOLD, "spaced_tiles_cases.json"))) if c["name"] != "sp_m1_k80_K32"]
 E2E = {c["name"]: c for c in json.load(open(os.path.join(GOLD, "e2e_cases.json")))}
-
-
-def md5(data):
-    return hashlib.md5(data).hexdigest()
-
-
-@pytest.fixture(scope="module")
-def host_walk(tmp_path_factory):
-    exe = str(tmp_path_factory.mktemp("hw") / "host_walk_spaced")
-    subprocess.run(["g++", "-std=c++17", "-O2", "-Wno-unknown-pragmas", "-o", exe,
-                    os.path.join(ROOT, "tests", "host_walk", "host_walk_spaced.cpp"), os.path.join(ROOT, "oracle", "abyss_oracle.c")],
-                   check=True, capture_output=True)
-    return exe
+host_walk = parity.harness("host_walk_spaced", "tests/host_walk/host_walk_spaced.cpp", parity.ORACLE)
 
 
 def _write_reads(tmp_path, suite, case):
@@ -65,9 +50,8 @@ def _write_reads(tmp_path, suite, case):
 
 def _walk(exe, tmp_path, case, reads, drop=None):
     log = str(tmp_path / "read.log")
-    r = subprocess.run([exe, str(case["k"]), str(case["kc"]), str(case["H"]), str(case["counters"]), str(case.get("trim", case["k"])),
-                        case["mask"], reads, log] + ([] if drop is None else [str(drop)]), capture_output=True)
-    assert r.returncode == 0, r.stderr.decode()
+    r = parity.run(exe, case["k"], case["kc"], case["H"], case["counters"], case.get("trim", case["k"]), case["mask"], reads, log,
+                   *([] if drop is None else [drop]))
     err = r.stderr.decode()
     m = re.search(r"(\d+) tiles from (\d+) markers.*\n.*?(\d+) tile splices, (\d+) serial fallbacks", err)
     assert m, err

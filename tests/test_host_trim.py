@@ -4,43 +4,33 @@ and qualities, the record writer), run on one thread by tests/host_trim, prints 
 tests/host_konnector, whose files are the reference's (tests/test_host_konnector.py).  On the hand-made graphs the trim
 lengths are also compared read by read with the ones the reference's output shows.  Case trim_quality runs the reader's -q
 through trim and expects what the reference prints for the file cut beforehand."""
-import hashlib
 import json
 import os
 import re
 import subprocess
-import sys
 
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GOLD = os.path.join(ROOT, "tests", "golden")
-sys.path.insert(0, GOLD)
-from make_golden_trim import FILTERS, fastq_records, write_inputs  # noqa: E402
+import parity
+from make_golden_trim import FILTERS, fastq_records, write_inputs
 
-CASES = [c for c in json.load(open(os.path.join(GOLD, "trim_cases.json"))) if "harness" in c]
+CASES = [c for c in json.load(open(os.path.join(parity.GOLD, "trim_cases.json"))) if "harness" in c]
 EXITS = ("end_no_vertex", "end_tip", "first_not_tip", "fork")
+host_konnector = parity.harness("host_konnector", "tests/host_konnector/host_konnector.cpp")
+host_trim = parity.harness("host_trim", "tests/host_trim/host_trim.cpp")
 
 
 @pytest.fixture(scope="module")
-def work(tmp_path_factory):
+def work(tmp_path_factory, host_konnector, host_trim):
     d = tmp_path_factory.mktemp("ht")
-    exes = {}
-    for name in ("host_konnector", "host_trim"):
-        exes[name] = str(d / name)
-        subprocess.run(["g++", "-std=c++17", "-O2", "-pthread", "-o", exes[name], os.path.join(ROOT, "tests", name, name + ".cpp")],
-                       check=True, capture_output=True)
     write_inputs(str(d))
     for f in FILTERS:
-        r = subprocess.run([exes["host_konnector"], *map(str, f["harness"])], cwd=str(d), capture_output=True)
-        assert r.returncode == 0, r.stderr.decode()
+        parity.run(host_konnector, *f["harness"], cwd=d)
     out = {}
     for c in CASES:
-        r = subprocess.run([exes["host_trim"], str(c["harness"][0]), "--lengths", "len.txt", *map(str, c["harness"][1:])], cwd=str(d),
-                           capture_output=True)
-        assert r.returncode == 0, r.stderr.decode()
-        out[c["name"]] = (hashlib.md5(r.stdout).hexdigest(), r.stderr.decode(), open(d / "len.txt").read().splitlines(), r.stdout)
-    out["dir"], out["exe"] = d, exes["host_trim"]
+        r = parity.run(host_trim, c["harness"][0], "--lengths", "len.txt", *c["harness"][1:], cwd=d)
+        out[c["name"]] = (parity.md5(r.stdout), r.stderr.decode(), open(d / "len.txt").read().splitlines(), r.stdout)
+    out["dir"], out["exe"] = d, host_trim
     return out
 
 

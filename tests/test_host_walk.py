@@ -11,18 +11,11 @@ import subprocess
 
 import pytest
 
+import parity
 from abyss_b200.synth import ReadSet
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GOLD = os.path.join(ROOT, "tests", "golden")
-
-
-@pytest.fixture(scope="module")
-def host_walk(tmp_path_factory):
-    exe = str(tmp_path_factory.mktemp("hw") / "host_walk")
-    subprocess.run(["g++", "-std=c++17", "-O2", "-Wno-unknown-pragmas", "-o", exe, os.path.join(ROOT, "tests", "host_walk", "host_walk.cpp"),
-                    os.path.join(ROOT, "oracle", "abyss_oracle.c")], check=True, capture_output=True)
-    return exe
+GOLD = parity.GOLD
+host_walk = parity.harness("host_walk", "tests/host_walk/host_walk.cpp", parity.ORACLE)
 
 
 def _reads(tmp_path, reads):
@@ -37,21 +30,11 @@ def _reads(tmp_path, reads):
     return out
 
 
-def _run(exe, k, kc, H, counters, trim, reads, mask="", tiles=False):
-    env = dict(os.environ, HOST_WALK_MASK=mask)
-    env.pop("HOST_WALK_TILES", None)
-    if tiles:
-        env["HOST_WALK_TILES"] = "1"
-    r = subprocess.run([exe, str(k), str(kc), str(H), str(counters), str(trim), reads], capture_output=True, text=True, env=env)
-    assert r.returncode == 0, r.stderr
-    return r.stdout
-
-
 @pytest.mark.parametrize("tiles", [False, True])
 def test_plain_kmers(host_walk, tmp_path, tiles):
     c = {c["name"]: c for c in json.load(open(os.path.join(GOLD, "e2e_cases.json")))}["e2e_g10k_k25_small"]
-    got = _run(host_walk, c["k"], c["kc"], c["H"], c["counters"], c["k"], _reads(tmp_path, c["name"]), tiles=tiles)
-    assert got == open(os.path.join(GOLD, c["name"] + ".fa")).read()
+    got, _, _ = parity.run_host_walk(host_walk, c, _reads(tmp_path, c["name"]), tiles=tiles)
+    assert got == open(os.path.join(GOLD, c["name"] + ".fa"), "rb").read()
 
 
 MASK_CASES = json.load(open(os.path.join(GOLD, "mask_cases.json")))
@@ -61,10 +44,9 @@ MASK_CASES = json.load(open(os.path.join(GOLD, "mask_cases.json")))
                                   ("mask_g20k_qr11", "mask_g10k_K5", "mask_tandem_qr15", "mask_hairpin_K10", "mask_circ_qr17")],
                          ids=lambda c: c["name"])
 def test_spaced_seeds(host_walk, tmp_path, case):
-    got = _run(host_walk, case["k"], case["kc"], case["H"], case["counters"], case["k"], _reads(tmp_path, case["reads"]),
-               mask=case["mask"])
-    want = open(os.path.join(GOLD, case["name"] + ".fa")).read()
-    assert got.count(">") == case["n_contigs"]
+    got, _, _ = parity.run_host_walk(host_walk, case, _reads(tmp_path, case["reads"]))
+    want = open(os.path.join(GOLD, case["name"] + ".fa"), "rb").read()
+    assert got.count(b">") == case["n_contigs"]
     assert got == want
 
 
@@ -94,10 +76,7 @@ def test_dropped_tiles_same_output(host_walk, tmp_path, name, seed):
     else:
         c = {c["name"]: c for c in json.load(open(os.path.join(GOLD, "e2e_cases.json")))}[name]
         reads, counters, trim = _reads(tmp_path, name), c["counters"], c["k"]
-    env = dict(os.environ, HOST_WALK_MASK="", HOST_WALK_TILES="1", HOST_WALK_DROP_TILES=str(seed))
-    r = subprocess.run([host_walk, str(c["k"]), str(c["kc"]), str(c["H"]), str(counters), str(trim), reads], capture_output=True,
-                       text=True, env=env)
-    assert r.returncode == 0, r.stderr
-    m = re.search(r"(\d+) dropped \((\d+) markers lost one tile, (\d+) all four\)", r.stderr)
-    assert m and int(m.group(2)) > 0 and int(m.group(3)) > 0, r.stderr
-    assert r.stdout == open(os.path.join(GOLD, name + ".fa")).read()
+    fasta, _, err = parity.run_host_walk(host_walk, dict(c, counters=counters, trim=trim), reads, drop=seed)
+    m = re.search(r"(\d+) dropped \((\d+) markers lost one tile, (\d+) all four\)", err)
+    assert m and int(m.group(2)) > 0 and int(m.group(3)) > 0, err
+    assert fasta == open(os.path.join(GOLD, name + ".fa"), "rb").read()

@@ -28,6 +28,7 @@
 #include <thrust/iterator/counting_iterator.h>
 #include <algorithm>
 #include <chrono>
+#include <cstddef>
 #include <cstdlib>
 #include <cstring>
 #include <new>
@@ -44,6 +45,45 @@ __host__ __device__ inline uint64_t tile_slot(uint64_t key, unsigned cls, unsign
 	return (((key ^ (0x9E3779B97F4A7C15ULL * (cls + 1))) * 0xD6E8FEB86659FD93ULL) >> 24) & mask;
 }
 
+/** device view of the tile store: the records and their (key, class) table, open addressing over mask + 1 entries that
+ *  hold a tile index + 1, 0 = empty (tab == nullptr: tiles disabled) */
+struct TileView {
+	TileRec* recs;
+	unsigned* tab;
+	unsigned mask;
+};
+
+/** enter tile idx, whose marker is (key, cls), into the table.  A palindromic marker gives the same (key, class) twice:
+ *  the first tile entered keeps the entry. */
+__device__ inline void tile_insert(const TileView& v, uint64_t key, unsigned cls, unsigned idx)
+{
+	for (uint64_t s = tile_slot(key, cls, v.mask);; s = (s + 1) & v.mask) {
+		const unsigned old = atomicCAS(v.tab + s, 0u, idx + 1);
+		if (old == 0u)
+			return;
+		const TileRec* o = v.recs + (old - 1);
+		if (o->key == key && o->cls == cls)
+			return;
+	}
+}
+
+/** the tile of (key, cls), nullptr if there is none; *entry gets its entry (tile index + 1).  The probe ends at the first
+ *  empty entry. */
+__device__ inline const TileRec* tile_find(const TileView& v, uint64_t key, unsigned cls, unsigned* entry = nullptr)
+{
+	for (uint64_t s = tile_slot(key, cls, v.mask);; s = (s + 1) & v.mask) {
+		const unsigned e = __ldcg(v.tab + s);
+		if (e == 0)
+			return nullptr;
+		const TileRec* t = v.recs + (e - 1);
+		if (t->key == key && t->cls == cls) {
+			if (entry)
+				*entry = e;
+			return t;
+		}
+	}
+}
+
 struct WarpCtx {
 	unsigned k, trim;
 	RollTab rt;
@@ -57,25 +97,12 @@ struct WarpCtx {
 	unsigned long long arena_size;
 	unsigned long long* arena_top;
 	unsigned fail_;
-	// tiles (null table = disabled)
-	const TileRec* tile_recs;
-	const unsigned* tile_tab; // open addressing: tile index + 1, 0 = empty
-	unsigned tile_mask;
+	TileView tiles; // the walks only read it
 
-	__device__ bool tiles_enabled() const { return tile_tab != nullptr; }
-	__device__ const TileRec* tile_lookup(uint64_t key, unsigned cls) const
-	{
-		for (uint64_t s = tile_slot(key, cls, tile_mask);; s = (s + 1) & tile_mask) {
-			const unsigned v = __ldcg(tile_tab + s);
-			if (v == 0)
-				return nullptr;
-			const TileRec* t = tile_recs + (v - 1);
-			if (t->key == key && t->cls == cls)
-				return t;
-		}
-	}
-	__device__ uint32_t tile_index(const TileRec* t) const { return (uint32_t)(t - tile_recs); }
-	__device__ const TileRec* tile_at(uint32_t idx) const { return tile_recs + idx; }
+	__device__ bool tiles_enabled() const { return tiles.tab != nullptr; }
+	__device__ const TileRec* tile_lookup(uint64_t key, unsigned cls) const { return tile_find(tiles, key, cls); }
+	__device__ uint32_t tile_index(const TileRec* t) const { return (uint32_t)(t - tiles.recs); }
+	__device__ const TileRec* tile_at(uint32_t idx) const { return tiles.recs + idx; }
 	__device__ void prefetch(const void* p) const
 	{
 		if (p)
@@ -323,11 +350,11 @@ struct WarpCtx {
 			// the warp sweeps one tile at a time with coalesced loads (8 hashes per lane in flight); the next tile's record
 			// and hashes are prefetched into L2 meanwhile, so a tile costs about one L2 round trip
 			for (unsigned ti = 0; ti < tv.n; ++ti) {
-				const TileRec* T = tile_recs + tv.p[ti];
+				const TileRec* T = tiles.recs + tv.p[ti];
 				if (ti + 2 < tv.n && lane == 0)
-					prefetch(tile_recs + tv.p[ti + 2]);
+					prefetch(tiles.recs + tv.p[ti + 2]);
 				if (ti + 1 < tv.n) {
-					const TileRec* Tn = tile_recs + tv.p[ti + 1];
+					const TileRec* Tn = tiles.recs + tv.p[ti + 1];
 					const uint64_t* thn = Tn->hashes;
 					if (lane * 16u < Tn->n)
 						prefetch(thn + lane * 16u);
@@ -438,13 +465,6 @@ struct WalkCfg {
 	const uint8_t* counters;
 };
 
-/** device view of the tile store (tab == nullptr: tiles disabled) */
-struct TileView {
-	const TileRec* recs;
-	const unsigned* tab;
-	unsigned mask;
-};
-
 __device__ __forceinline__ WarpCtx make_ctx(const WalkCfg& w, const HashCfg* cfg, Frame* frames, uint64_t* look, unsigned gwarp,
                                             uint8_t* arena, unsigned long long arena_size, unsigned long long* arena_top)
 {
@@ -462,9 +482,9 @@ __device__ __forceinline__ WarpCtx make_ctx(const WalkCfg& w, const HashCfg* cfg
 	c.arena_size = arena_size;
 	c.arena_top = arena_top;
 	c.fail_ = 0;
-	c.tile_recs = nullptr;
-	c.tile_tab = nullptr;
-	c.tile_mask = 0;
+	c.tiles.recs = nullptr; // field by field: a copy of the whole TileView also copies its padding (stack stores)
+	c.tiles.tab = nullptr;
+	c.tiles.mask = 0;
 	return c;
 }
 
@@ -580,9 +600,9 @@ k_extend(const uint8_t* __restrict__ bases, const uint64_t* __restrict__ offs, c
 	if (gwarp >= n_spec)
 		return;
 	WarpCtx c = make_ctx(w, &cfg, frames, look, gwarp, arena, arena_size, arena_top);
-	c.tile_recs = tv.recs;
-	c.tile_tab = tv.tab;
-	c.tile_mask = tv.mask;
+	c.tiles.recs = tv.recs; // field by field, as in make_ctx
+	c.tiles.tab = tv.tab;
+	c.tiles.mask = tv.mask;
 	const unsigned r = spec[gwarp];
 	const uint64_t beg = offs[r];
 	const unsigned L = (unsigned)(offs[r + 1] - beg);
@@ -639,11 +659,18 @@ k_find_markers(const uint64_t* __restrict__ key, const uint8_t* __restrict__ val
 	}
 }
 
+/** the counters of tile production.  `stored` comes first: every batch clears the words after it. */
+struct TileCounters {
+	unsigned stored;      // tiles given a record index; more than the capacity when records ran out
+	unsigned work;        // next work item of k_make_tiles
+	unsigned new_markers; // fresh markers of the batch, counted beyond the new-marker list too
+	unsigned no_room;     // marker windows the marker set had no room for
+	unsigned dropped;     // tiles computed but not stored: the records or the pool were full
+};
+
 struct TileStore { // device-side handles used while producing tiles
-	TileRec* recs;
-	unsigned* tab;
-	unsigned mask;
-	unsigned cap;          // capacity of recs
+	TileView v;
+	unsigned cap; // capacity of v.recs
 	unsigned* n_recs;
 	uint8_t* pool;
 	unsigned long long pool_size;
@@ -705,16 +732,9 @@ k_make_tiles(const uint8_t* __restrict__ bases, const uint64_t* __restrict__ off
 		t.bases = db;
 		__syncwarp();
 		if (c.lane == 0) {
-			ts.recs[idx] = t;
+			ts.v.recs[idx] = t;
 			__threadfence();
-			for (uint64_t s = tile_slot(t.key, t.cls, ts.mask);; s = (s + 1) & ts.mask) {
-				const unsigned old = atomicCAS(ts.tab + s, 0u, idx + 1);
-				if (old == 0u)
-					break;
-				const TileRec* o = ts.recs + (old - 1);
-				if (o->key == t.key && o->cls == t.cls)
-					break; // palindromic marker: the same (key, class) twice, keep the first
-			}
+			tile_insert(ts.v, t.key, t.cls, idx);
 		}
 	}
 }
@@ -737,46 +757,30 @@ k_export_tiles(const TileRec* __restrict__ recs, unsigned first, unsigned n, con
 /** received tiles [first, first + n) (pool offsets relative to the sender's segment, which now lives at seg_base):
  *  rebase the pointers and enter them into the (marker, class) table */
 __global__ void __launch_bounds__(256)
-k_import_tiles(TileRec* __restrict__ recs, unsigned first, unsigned n, uint8_t* seg_base, unsigned* __restrict__ tab, unsigned mask)
+k_import_tiles(TileView tv, unsigned first, unsigned n, uint8_t* seg_base)
 {
 	const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
 	if (i >= n)
 		return;
-	TileRec* t = recs + first + i;
+	TileRec* t = tv.recs + first + i;
 	t->bases = seg_base + reinterpret_cast<uintptr_t>(t->bases);
 	t->hashes = reinterpret_cast<uint64_t*>(seg_base + reinterpret_cast<uintptr_t>(t->hashes));
 	t->next = 0;
-	for (uint64_t s = tile_slot(t->key, t->cls, mask);; s = (s + 1) & mask) {
-		const unsigned old = atomicCAS(tab + s, 0u, first + i + 1);
-		if (old == 0u)
-			break;
-		const TileRec* o = recs + (old - 1);
-		if (o->key == t->key && o->cls == t->cls)
-			break;
-	}
+	tile_insert(tv, t->key, t->cls, first + i);
 }
 
 /** resolve TileRec::next for every tile that ended on a marker (tiles of later batches link to earlier ones
  *  and vice versa, so this runs over the whole store after each production) */
 __global__ void __launch_bounds__(256)
-k_link_tiles(TileRec* recs, unsigned n, const unsigned* __restrict__ tab, unsigned mask)
+k_link_tiles(TileView tv, unsigned n)
 {
 	for (unsigned i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-		TileRec* t = recs + i;
+		TileRec* t = tv.recs + i;
 		if (t->next || t->stop_kind != TS_MARKER || t->n == 0)
 			continue;
-		const uint64_t key = t->end_key;
-		const unsigned cls = ((unsigned)t->end_orient << 1) | (t->cls & 1u);
-		for (uint64_t s = tile_slot(key, cls, mask);; s = (s + 1) & mask) {
-			const unsigned v = tab[s];
-			if (v == 0)
-				break;
-			const TileRec* o = recs + (v - 1);
-			if (o->key == key && o->cls == cls) {
-				t->next = v;
-				break;
-			}
-		}
+		unsigned e;
+		if (tile_find(tv, t->end_key, ((unsigned)t->end_orient << 1) | (t->cls & 1u), &e))
+			t->next = e;
 	}
 }
 
@@ -1167,13 +1171,45 @@ k_replay_all(ReplayIO io, unsigned n_contigs, const unsigned* __restrict__ big, 
 	}
 }
 
+// =============================================================================================
+// host side
+// =============================================================================================
+/** the tile store (abb_walk.cuh "Tiles"), kept across batches, and the scratch of tile production.  ensure_tile_store
+ *  builds it whole, sized from the solid filter; abb_assembler_reset clears it. */
+struct Tiles {
+	DevBuf<TileRec> recs;
+	unsigned cap = 0;
+	DevBuf<unsigned> tab; // the (key, class) table of TileView; a power of two entries
+	DevBuf<TileCounters> n;
+	DevBuf<uint8_t> pool; // the bases and hashes of the records
+	unsigned long long pool_size = 0;
+	DevBuf<unsigned long long> pool_top;
+	DevBuf<unsigned long long> marker_set; // marker_set_insert; a power of two entries
+	// production scratch
+	DevBuf<unsigned long long> new_markers;
+	DevBuf<uint64_t> key_h0;   // spaced seed only: unmasked canonical hash (tile_key) of every window of the batch
+	DevBuf<uint8_t> key_valid; // and whether all k bases of the window are ACGT
+	DevBuf<TileRec> tile_export;
+	DevBuf<uint8_t> stage_bases;
+	DevBuf<uint64_t> stage_hashes;
+
+	TileView view() const { return { recs.p, tab.p, (unsigned)(tab.cap - 1) }; }
+	unsigned marker_set_mask() const { return (unsigned)(marker_set.cap - 1); }
+	/** an empty store: no tiles, no markers */
+	int clear(cudaStream_t st) const
+	{
+		ABB_CUDA(cudaMemsetAsync(tab.p, 0, tab.cap * sizeof(unsigned), st));
+		ABB_CUDA(cudaMemsetAsync(marker_set.p, 0, marker_set.cap * sizeof(unsigned long long), st));
+		ABB_CUDA(cudaMemsetAsync(n.p, 0, sizeof(TileCounters), st));
+		ABB_CUDA(cudaMemsetAsync(pool_top.p, 0, sizeof(unsigned long long), st));
+		return ABB_OK;
+	}
+};
+
 } // namespace abb
 
 using namespace abb;
 
-// =============================================================================================
-// host side
-// =============================================================================================
 struct abb_assembler {
 	abb_filter* solid = nullptr; // not owned
 	std::unique_ptr<abb_filter, decltype(&abb_filter_destroy)> assembled{ nullptr, abb_filter_destroy };
@@ -1194,6 +1230,8 @@ struct abb_assembler {
 	DevBuf<uint64_t> offs, slot_offs, h0, coffs, cslot, ch0;
 	DevBuf<unsigned> cand, spec, spec_cbeg, clen, ccov, status, seg_contig, seg_len, big_idx, big_spec;
 	DevBuf<uint64_t> seg_beg, seg_slot, rep_off;
+	DevBuf<unsigned long long> rep_tab;
+	DevBuf<uint8_t> rep_flag;
 	DevBuf<ContigRec> recs, recs_sorted;
 	DevBuf<Frame> frames;
 	DevBuf<uint64_t> look;
@@ -1208,24 +1246,8 @@ struct abb_assembler {
 	DevBuf<unsigned> d_ends_n;
 	uint64_t ends_upper = 0; // upper bound on entries
 
-	// tile store (abb_walk.cuh "Tiles"); persistent across batches
 	bool tiles_on = true;
-	DevBuf<TileRec> d_tiles;
-	unsigned tile_cap = 0;
-	DevBuf<unsigned> d_tile_tab;
-	unsigned tile_tab_mask = 0;
-	DevBuf<unsigned> d_tile_n; // [0] tiles stored, [1] work counter, [2] new markers, [3] markers without room, [4] tiles dropped
-	DevBuf<uint8_t> d_tile_pool;
-	unsigned long long tile_pool_size = 0;
-	DevBuf<unsigned long long> d_tile_pool_top;
-	DevBuf<unsigned long long> d_marker_set;
-	unsigned marker_set_mask = 0;
-	DevBuf<unsigned long long> new_markers, rep_tab;
-	DevBuf<uint64_t> key_h0;  // spaced seed only: unmasked canonical hash (tile_key) of every window of the batch
-	DevBuf<uint8_t> key_valid; // and whether all k bases of the window are ACGT
-	DevBuf<TileRec> tile_export;
-	DevBuf<uint8_t> stage_bases, rep_flag;
-	DevBuf<uint64_t> stage_hashes;
+	std::unique_ptr<Tiles> tiles; // null until the first batch that produces tiles
 
 	// speculation control
 	unsigned spec_target = 512;
@@ -1249,7 +1271,6 @@ struct abb_assembler {
 namespace {
 
 constexpr unsigned kMaxSpec = 1024;
-constexpr unsigned kTileCounters = 5; // the words of abb_assembler::d_tile_n
 constexpr unsigned kMinSpec = 256;   // with tiles a round costs about the same latency for 64 or 1024 walkers, and wasted walks are cheap
 constexpr unsigned long long kArenaDefault = 4ULL << 30;
 static unsigned long long g_arena_hint = 0; // the arena size the previous assembler of this process ended up needing
@@ -1358,21 +1379,10 @@ int allgather_slices(abb_assembler* a, const uint8_t* mine, uint64_t n_total, ui
 	return ABB_OK;
 }
 
-TileView tile_view(const abb_assembler* a, bool on)
-{
-	TileView v = { nullptr, nullptr, 0 };
-	if (on && a->tiles_on && a->d_tile_tab.p) {
-		v.recs = a->d_tiles.p;
-		v.tab = a->d_tile_tab.p;
-		v.mask = a->tile_tab_mask;
-	}
-	return v;
-}
-
 /** allocate the tile store on first use, sized from the number of solid k-mers in the filter */
 int ensure_tile_store(abb_assembler* a)
 {
-	if (a->d_tile_tab.p || !a->tiles_on)
+	if (a->tiles || !a->tiles_on)
 		return ABB_OK;
 	uint64_t nz = 0, th = 0;
 	ABB_CHECK(abb_filter_popcount(a->solid, &nz, &th));
@@ -1388,31 +1398,21 @@ int ensure_tile_store(abb_assembler* a)
 	uint64_t mset = 1;
 	while (mset < markers * 4)
 		mset <<= 1;
-	// the store takes the six pieces only once all of them exist: a store with d_tile_tab set counts as complete
-	DevBuf<TileRec> tiles;
-	DevBuf<unsigned> tile_tab, tile_n;
-	DevBuf<unsigned long long> marker_set, pool_top;
-	DevBuf<uint8_t> tile_pool;
-	ABB_CHECK(tiles.alloc(tile_cap));
-	ABB_CHECK(tile_tab.alloc(tab));
-	ABB_CUDA(cudaMemsetAsync(tile_tab.p, 0, tab * sizeof(unsigned), a->stream));
-	ABB_CHECK(marker_set.alloc(mset));
-	ABB_CUDA(cudaMemsetAsync(marker_set.p, 0, mset * sizeof(unsigned long long), a->stream));
-	ABB_CHECK(tile_pool.alloc(pool));
-	ABB_CHECK(tile_n.alloc(kTileCounters));
-	ABB_CUDA(cudaMemsetAsync(tile_n.p, 0, kTileCounters * sizeof(unsigned), a->stream));
-	ABB_CHECK(pool_top.alloc(1));
-	ABB_CUDA(cudaMemsetAsync(pool_top.p, 0, sizeof(unsigned long long), a->stream));
-	a->d_tiles = std::move(tiles);
-	a->tile_cap = tile_cap;
-	a->d_tile_tab = std::move(tile_tab);
-	a->tile_tab_mask = (unsigned)(tab - 1);
-	a->d_marker_set = std::move(marker_set);
-	a->marker_set_mask = (unsigned)(mset - 1);
-	a->d_tile_pool = std::move(tile_pool);
-	a->tile_pool_size = pool;
-	a->d_tile_n = std::move(tile_n);
-	a->d_tile_pool_top = std::move(pool_top);
+	std::unique_ptr<Tiles> t(new (std::nothrow) Tiles());
+	if (!t) {
+		set_error("out of host memory");
+		return ABB_ENOMEM;
+	}
+	ABB_CHECK(t->recs.alloc(tile_cap));
+	t->cap = tile_cap;
+	ABB_CHECK(t->tab.alloc(tab));
+	ABB_CHECK(t->marker_set.alloc(mset));
+	ABB_CHECK(t->pool.alloc(pool));
+	t->pool_size = pool;
+	ABB_CHECK(t->n.alloc(1));
+	ABB_CHECK(t->pool_top.alloc(1));
+	ABB_CHECK(t->clear(a->stream));
+	a->tiles = std::move(t); // only once every piece exists
 	return ABB_OK;
 }
 
@@ -1420,6 +1420,7 @@ int ensure_tile_store(abb_assembler* a)
  *  rank and theirs are appended here; afterwards every rank holds all tiles (indices differ between ranks, content not) */
 int exchange_tiles(abb_assembler* a, unsigned n0, unsigned n1, unsigned long long p0, unsigned long long p1)
 {
+	Tiles& T = *a->tiles;
 	cudaStream_t st = a->stream;
 	const unsigned world = a->world(), rank = a->rank();
 	// 1. how much does everybody have?
@@ -1443,24 +1444,24 @@ int exchange_tiles(abb_assembler* a, unsigned n0, unsigned n1, unsigned long lon
 		nt += all[2 * r];
 		pt += (all[2 * r + 1] + 15) & ~15ULL;
 	}
-	ABB_REQUIRE(nt <= a->tile_cap && pt <= a->tile_pool_size, "tile store too small for the merged tiles (%llu tiles, %llu pool bytes)", nt, pt);
+	ABB_REQUIRE(nt <= T.cap && pt <= T.pool_size, "tile store too small for the merged tiles (%llu tiles, %llu pool bytes)", nt, pt);
 	// 3. my records with pool-relative pointers, then the two exchanges
-	ABB_CHECK(a->tile_export.reserve((size_t)(n1 - n0) + 1));
+	ABB_CHECK(T.tile_export.reserve((size_t)(n1 - n0) + 1));
 	if (n1 > n0)
-		k_export_tiles<<<blocks_for(n1 - n0, 256), 256, 0, st>>>(a->d_tiles.p, n0, n1 - n0, a->d_tile_pool.p + p0, a->tile_export.p);
+		k_export_tiles<<<blocks_for(n1 - n0, 256), 256, 0, st>>>(T.recs.p, n0, n1 - n0, T.pool.p + p0, T.tile_export.p);
 	ABB_CUDA(cudaGetLastError());
-	ABB_CHECK(abb_comm_exchange_bytes(a->comm, a->tile_export.p, (uint64_t)(n1 - n0) * sizeof(TileRec), a->d_tiles.p, rec_off.data(), rec_bytes.data(), st));
-	ABB_CHECK(abb_comm_exchange_bytes(a->comm, a->d_tile_pool.p + p0, p1 - p0, a->d_tile_pool.p, pool_off.data(), pool_bytes.data(), st));
+	ABB_CHECK(abb_comm_exchange_bytes(a->comm, T.tile_export.p, (uint64_t)(n1 - n0) * sizeof(TileRec), T.recs.p, rec_off.data(), rec_bytes.data(), st));
+	ABB_CHECK(abb_comm_exchange_bytes(a->comm, T.pool.p + p0, p1 - p0, T.pool.p, pool_off.data(), pool_bytes.data(), st));
 	for (unsigned r = 0; r < world; ++r) {
 		if (r == rank || all[2 * r] == 0)
 			continue;
 		const unsigned first = (unsigned)(rec_off[r] / sizeof(TileRec)), n = (unsigned)all[2 * r];
-		k_import_tiles<<<blocks_for(n, 256), 256, 0, st>>>(a->d_tiles.p, first, n, a->d_tile_pool.p + pool_off[r], a->d_tile_tab.p, a->tile_tab_mask);
+		k_import_tiles<<<blocks_for(n, 256), 256, 0, st>>>(T.view(), first, n, T.pool.p + pool_off[r]);
 	}
 	ABB_CUDA(cudaGetLastError());
 	const unsigned nt32 = (unsigned)nt;
-	ABB_CUDA(cudaMemcpyAsync(a->d_tile_n.p, &nt32, sizeof nt32, cudaMemcpyHostToDevice, st));
-	ABB_CUDA(cudaMemcpyAsync(a->d_tile_pool_top.p, &pt, sizeof pt, cudaMemcpyHostToDevice, st));
+	ABB_CUDA(cudaMemcpyAsync(&T.n.p->stored, &nt32, sizeof nt32, cudaMemcpyHostToDevice, st));
+	ABB_CUDA(cudaMemcpyAsync(T.pool_top.p, &pt, sizeof pt, cudaMemcpyHostToDevice, st));
 	ABB_CUDA(cudaStreamSynchronize(st));
 	a->st.launches += 2 + world;
 	return ABB_OK;
@@ -1473,36 +1474,37 @@ int produce_tiles(abb_assembler* a, uint64_t n_reads, uint64_t n_slots)
 		return ABB_OK;
 	StreamTimer tt = a->time_phase(&a->st.ms_tiles);
 	ABB_CHECK(ensure_tile_store(a));
+	Tiles& T = *a->tiles;
 	abb_filter* f = a->solid;
 	cudaStream_t st = a->stream;
 	const WalkCfg w = walk_cfg(a);
 	const unsigned world = a->world(), rank = a->rank();
-	const unsigned out_cap = (unsigned)std::min<uint64_t>(n_slots / (kMarkerMask + 1) * 2 + 4096, a->marker_set_mask / 2 + 1);
-	ABB_CHECK(a->new_markers.reserve(out_cap));
-	ABB_CUDA(cudaMemsetAsync(a->d_tile_n.p + 1, 0, (kTileCounters - 1) * sizeof(unsigned), st));
+	const unsigned out_cap = (unsigned)std::min<uint64_t>(n_slots / (kMarkerMask + 1) * 2 + 4096, T.marker_set_mask() / 2 + 1);
+	ABB_CHECK(T.new_markers.reserve(out_cap));
+	ABB_CUDA(cudaMemsetAsync(&T.n.p->work, 0, sizeof(TileCounters) - offsetof(TileCounters, work), st)); // all but `stored`
 	const uint64_t* key = a->h0.p;
 	const uint8_t* key_valid = a->valid.p;
 	if (a->rt.nmask) {
 		// spaced seed: h0 is the masked Bloom hash and valid covers only the '1' positions, but markers are named by the full
 		// k-mer.  One more streaming pass of the unmasked K1 over the batch gives each window its tile_key and full validity.
-		ABB_CHECK(a->key_h0.reserve(n_slots + 1));
-		ABB_CHECK(a->key_valid.reserve(n_slots + 1));
-		ABB_CHECK(launch_hash(f->k, nullptr, a->cur_bases, a->cur_offs, a->slot_offs.p, 0, n_reads, 0, a->key_h0.p, a->key_valid.p, st,
+		ABB_CHECK(T.key_h0.reserve(n_slots + 1));
+		ABB_CHECK(T.key_valid.reserve(n_slots + 1));
+		ABB_CHECK(launch_hash(f->k, nullptr, a->cur_bases, a->cur_offs, a->slot_offs.p, 0, n_reads, 0, T.key_h0.p, T.key_valid.p, st,
 		                      &a->st.launches));
-		key = a->key_h0.p;
-		key_valid = a->key_valid.p;
+		key = T.key_h0.p;
+		key_valid = T.key_valid.p;
 	}
-	k_find_markers<<<a->sms * 16, 256, 0, st>>>(key, key_valid, a->h0.p, a->slot_offs.p, n_reads, n_slots, w, f->cfg, a->d_marker_set.p,
-	                                         a->marker_set_mask, a->new_markers.p, a->d_tile_n.p + 2, out_cap, a->d_tile_n.p + 3,
+	k_find_markers<<<a->sms * 16, 256, 0, st>>>(key, key_valid, a->h0.p, a->slot_offs.p, n_reads, n_slots, w, f->cfg, T.marker_set.p,
+	                                         T.marker_set_mask(), T.new_markers.p, &T.n.p->new_markers, out_cap, &T.n.p->no_room,
 	                                         world, rank);
 	ABB_CUDA(cudaGetLastError());
-	unsigned tn[kTileCounters] = {};
+	TileCounters tn = {};
 	unsigned long long p0 = 0;
-	ABB_CUDA(cudaMemcpyAsync(tn, a->d_tile_n.p, sizeof tn, cudaMemcpyDeviceToHost, st));
-	ABB_CUDA(cudaMemcpyAsync(&p0, a->d_tile_pool_top.p, sizeof p0, cudaMemcpyDeviceToHost, st));
+	ABB_CUDA(cudaMemcpyAsync(&tn, T.n.p, sizeof tn, cudaMemcpyDeviceToHost, st));
+	ABB_CUDA(cudaMemcpyAsync(&p0, T.pool_top.p, sizeof p0, cudaMemcpyDeviceToHost, st));
 	ABB_CUDA(cudaStreamSynchronize(st));
-	const unsigned nm = std::min(tn[2], out_cap), n0 = std::min(tn[0], a->tile_cap);
-	a->st.untiled_markers += tn[3] + (tn[2] - nm); // no room in the marker set, or beyond the new-marker list
+	const unsigned nm = std::min(tn.new_markers, out_cap), n0 = std::min(tn.stored, T.cap);
+	a->st.untiled_markers += tn.no_room + (tn.new_markers - nm); // no room in the marker set, or beyond the new-marker list
 	a->st.launches += 1;
 	if (nm == 0 && world == 1)
 		return ABB_OK;
@@ -1511,32 +1513,31 @@ int produce_tiles(abb_assembler* a, uint64_t n_reads, uint64_t n_slots)
 		const unsigned grid = std::min(blocks_for((uint64_t)nm * 4, kWalkWarps), a->tile_ctas);
 		const unsigned warps = grid * kWalkWarps;
 		ABB_CHECK(ensure_scratch(a, warps));
-		ABB_CHECK(a->stage_bases.reserve((size_t)warps * kTileCap));
-		ABB_CHECK(a->stage_hashes.reserve((size_t)warps * kTileCap));
-		TileStore ts = { a->d_tiles.p, a->d_tile_tab.p, a->tile_tab_mask, a->tile_cap, a->d_tile_n.p, a->d_tile_pool.p, a->tile_pool_size,
-			             a->d_tile_pool_top.p };
-		ABB_DISPATCH_KW(a->kw, (k_make_tiles<KW><<<grid, kWalkWarps * 32, 0, st>>>(a->cur_bases, a->cur_offs, a->new_markers.p, nm,
-		                                                                          a->d_tile_n.p + 1, w, f->cfg, a->frames.p, a->look.p,
-		                                                                          a->stage_bases.p, a->stage_hashes.p, ts, a->d_tile_n.p + 4)));
+		ABB_CHECK(T.stage_bases.reserve((size_t)warps * kTileCap));
+		ABB_CHECK(T.stage_hashes.reserve((size_t)warps * kTileCap));
+		const TileStore ts = { T.view(), T.cap, &T.n.p->stored, T.pool.p, T.pool_size, T.pool_top.p };
+		ABB_DISPATCH_KW(a->kw, (k_make_tiles<KW><<<grid, kWalkWarps * 32, 0, st>>>(a->cur_bases, a->cur_offs, T.new_markers.p, nm, &T.n.p->work, w, f->cfg,
+		                                                                          a->frames.p, a->look.p, T.stage_bases.p, T.stage_hashes.p, ts,
+		                                                                          &T.n.p->dropped)));
 		ABB_CUDA(cudaGetLastError());
 		a->st.launches += 1;
 	}
 	unsigned long long p1 = 0;
-	ABB_CUDA(cudaMemcpyAsync(tn, a->d_tile_n.p, sizeof tn, cudaMemcpyDeviceToHost, st));
-	ABB_CUDA(cudaMemcpyAsync(&p1, a->d_tile_pool_top.p, sizeof p1, cudaMemcpyDeviceToHost, st));
+	ABB_CUDA(cudaMemcpyAsync(&tn, T.n.p, sizeof tn, cudaMemcpyDeviceToHost, st));
+	ABB_CUDA(cudaMemcpyAsync(&p1, T.pool_top.p, sizeof p1, cudaMemcpyDeviceToHost, st));
 	ABB_CUDA(cudaStreamSynchronize(st));
-	unsigned nt = std::min(tn[0], a->tile_cap);
-	a->st.dropped_tiles += tn[4];
-	p1 = std::min(p1, a->tile_pool_size);
+	unsigned nt = std::min(tn.stored, T.cap);
+	a->st.dropped_tiles += tn.dropped;
+	p1 = std::min(p1, T.pool_size);
 	a->st.markers += nm;
 	a->st.tiles = nt;
 	if (world > 1) {
 		ABB_CHECK(exchange_tiles(a, n0, nt, p0, p1));
-		ABB_CUDA(cudaMemcpyAsync(&nt, a->d_tile_n.p, sizeof nt, cudaMemcpyDeviceToHost, st));
+		ABB_CUDA(cudaMemcpyAsync(&nt, &T.n.p->stored, sizeof nt, cudaMemcpyDeviceToHost, st));
 		ABB_CUDA(cudaStreamSynchronize(st));
 		a->st.tiles = nt;
 	}
-	k_link_tiles<<<a->sms * 8, 256, 0, st>>>(a->d_tiles.p, (unsigned)a->st.tiles, a->d_tile_tab.p, a->tile_tab_mask);
+	k_link_tiles<<<a->sms * 8, 256, 0, st>>>(T.view(), (unsigned)a->st.tiles);
 	ABB_CUDA(cudaGetLastError());
 	a->st.launches += 1;
 	return ABB_OK;
@@ -1564,7 +1565,7 @@ int run_extend(abb_assembler* a, unsigned n_spec, bool use_tiles, bool keep_aren
 		ABB_CUDA(cudaMemcpyAsync(a->d_arena_top.p, &arena_mark, sizeof arena_mark, cudaMemcpyHostToDevice, st));
 		ABB_CUDA(cudaMemsetAsync(a->d_nrecs.p, 0, sizeof(unsigned), st));
 		const WalkCfg w = walk_cfg(a);
-		const TileView tv = tile_view(a, use_tiles);
+		const TileView tv = use_tiles && a->tiles ? a->tiles->view() : TileView{};
 		StreamTimer tw = a->time_inner(&a->st.ms_walk); // read where this turn of the loop ends, after the synchronise below
 		ABB_DISPATCH_KW(a->kw, (k_extend<KW><<<blocks_for(n_spec, kWalkWarps), kWalkWarps * 32, 0, st>>>(
 		                           a->cur_bases, a->cur_offs, a->spec.p, n_spec, w, f->cfg, a->frames.p, a->look.p, a->d_arena.p, a->arena_size,
@@ -1761,7 +1762,7 @@ int extend_tiled(abb_assembler* a, Round& r)
 /** repeat check on everything that was produced with tiles: a read one of whose paths repeats a vertex is to be redone */
 int check_repeats(abb_assembler* a, Round& r)
 {
-	if (!a->tiles_on || !a->d_tile_tab.p)
+	if (!a->tiles)
 		return ABB_OK;
 	cudaStream_t st = a->stream;
 	std::vector<unsigned>& redo = r.redo;
@@ -2229,12 +2230,8 @@ int abb_assembler_reset(abb_assembler* a)
 		ABB_CUDA(cudaMemsetAsync(a->d_ends.p, 0, (size_t)a->ends_cap * sizeof(unsigned long long), st));
 	ABB_CUDA(cudaMemsetAsync(a->d_ends_n.p, 0, 2 * sizeof(unsigned), st));
 	a->ends_upper = 0;
-	if (a->d_tile_tab.p) { // the tiles describe the old contents of the solid filter: forget them, keep the memory
-		ABB_CUDA(cudaMemsetAsync(a->d_tile_tab.p, 0, ((size_t)a->tile_tab_mask + 1) * sizeof(unsigned), st));
-		ABB_CUDA(cudaMemsetAsync(a->d_marker_set.p, 0, ((size_t)a->marker_set_mask + 1) * sizeof(unsigned long long), st));
-		ABB_CUDA(cudaMemsetAsync(a->d_tile_n.p, 0, kTileCounters * sizeof(unsigned), st));
-		ABB_CUDA(cudaMemsetAsync(a->d_tile_pool_top.p, 0, sizeof(unsigned long long), st));
-	}
+	if (a->tiles) // the tiles describe the old contents of the solid filter: forget them, keep the memory
+		ABB_CHECK(a->tiles->clear(st));
 	ABB_CUDA(cudaStreamSynchronize(st));
 	a->counters = abb_assembly_counters{};
 	a->reads_seen = 0;
